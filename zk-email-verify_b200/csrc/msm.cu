@@ -5,8 +5,8 @@
 //   classify   : scalars 0 / points at infinity are dropped, scalars == 1 go to a "ones" list that is summed by a
 //                plain tree reduction (>= 90 % of EmailVerifier witness scalars are bits, SURVEY 8(d)), the rest
 //                go to the Pippenger list.
-//   pippenger  : signed c-bit digits -> histogram -> exclusive scan -> scatter of point indices by bucket
-//                (counting sort, no comparison sort) -> buckets cut into chunks of at most CHUNK entries so that a
+//   pippenger  : signed c-bit digits -> point indices sorted by bucket (counting sort, in two levels for large
+//                bucket sets: msm_sort.cuh) -> buckets cut into chunks of at most CHUNK entries so that a
 //                heavy bucket (small-valued witness scalars pile into few buckets) is spread over many threads ->
 //                per-chunk XYZZ accumulation with coalesced 32/64-byte affine point loads -> per-group running sums
 //                -> per-window tree reduction -> Horner over windows.
@@ -15,11 +15,13 @@
 #include "device_engine.cuh"
 #include "msm.cuh"
 #include "msm_ba.cuh"
+#include "msm_sort.cuh"
 #if defined(ZKE_MSM_G1)
 #include "msm_tc.cuh"
 #endif
 #include <algorithm>
 #include <cstdlib>
+#include <stdexcept>
 
 namespace zke {
 namespace dev {
@@ -142,8 +144,186 @@ __device__ __forceinline__ void for_each_digit(Fr s, const Digits& D, Fn f) {
     }
 }
 
+// ---------------------------------------------------------------- bucket sort of the digits (msm_sort.cuh)
+// Output: hist[b] entries in bucket b, offsets[b] = exclusive scan of hist (offsets[n_buckets] = total), entries in
+// bucket order, each (window * window_point_stride + point index) | sign << 31.  The order inside a bucket is not fixed.
+// A one-level counting sort costs one global atomic and one 4-byte write to a random place in a 200+ MB array per
+// digit (13 x 2^22 digits for the H MSM): every store of a warp lands in 32 different sectors, and the L2 write
+// transactions, not the bytes, set its time.  Both scatter passes below therefore first sort a block's digits in
+// shared memory and then store them in runs: consecutive threads write consecutive words of a partition (coarse pass,
+// ~26 digits per partition and block for the H MSM) or of a bucket (fine pass, ~8 per bucket and tile).
+static const int SORT_PART_BITS = 8;
+static const uint32_t SORT_PARTS = 1u << SORT_PART_BITS;
+static const int SORT_MAX_FINE_BITS = 11;     // buckets per partition: n_buckets <= 2^19
+static const int SORT_THREADS = 256;          // coarse passes, fine count pass
+static const int SORT_FINE_THREADS = 512;     // fine scatter pass
+static const uint32_t SORT_STAGE = 6656;      // digits a coarse block stages (6 B each): 512 scalars x 13 windows
+static const uint32_t SORT_TILE = 16384;      // digits of a fine tile
+// the one-level counting sort is faster for small bucket sets (the witness MSMs: 4096 buckets), whose histogram and
+// scatter targets stay in L2, and it needs fewer launches
+static const uint32_t SORT_TWO_LEVEL_MIN_BUCKETS = 1u << 16;
+// dynamic shared memory of the fine scatter pass: bin offsets, cursors and global positions, scan scratch, the tile
+static const size_t SORT_FINE_SMEM = 4 * (3 * ((size_t)1 << SORT_MAX_FINE_BITS) + 1 + SORT_FINE_THREADS + SORT_TILE);
+
+// in-place exclusive scan of s[0, n) by the whole block (tmp: THREADS words); s[n] = the total.  Ends synchronised.
+template <int THREADS>
+__device__ __forceinline__ void block_exclusive_scan(uint32_t* s, uint32_t n, uint32_t* tmp) {
+    const uint32_t per = (n + THREADS - 1) / THREADS, beg = min(n, threadIdx.x * per), end = min(n, beg + per);
+    uint32_t local = 0;
+    for (uint32_t i = beg; i < end; ++i) local += s[i];
+    tmp[threadIdx.x] = local;
+    __syncthreads();
+    for (uint32_t off = 1; off < THREADS; off <<= 1) {
+        const uint32_t v = threadIdx.x >= off ? tmp[threadIdx.x - off] : 0;
+        __syncthreads();
+        tmp[threadIdx.x] += v;
+        __syncthreads();
+    }
+    uint32_t run = tmp[threadIdx.x] - local;
+    for (uint32_t i = beg; i < end; ++i) { const uint32_t v = s[i]; s[i] = run; run += v; }
+    if (threadIdx.x == THREADS - 1) s[n] = tmp[THREADS - 1];
+    __syncthreads();
+}
+
+// mat[part][block] = the block's digits per partition; block k takes scalars [k * tile, (k + 1) * tile) of the list
+static __global__ void __launch_bounds__(SORT_THREADS)
+sort_coarse_count_kernel(const uint8_t* __restrict__ scalars, const uint32_t* __restrict__ list, const uint32_t* __restrict__ count_ptr,
+                         uint32_t count_fixed, Digits D, int fine_bits, uint32_t n_parts, uint32_t tile, uint32_t* mat) {
+    __shared__ uint32_t s_bin[SORT_PARTS];
+    const uint32_t count = count_ptr ? *count_ptr : count_fixed;
+    for (uint32_t i = threadIdx.x; i < n_parts; i += SORT_THREADS) s_bin[i] = 0;
+    __syncthreads();
+    const uint32_t beg = blockIdx.x * tile, end = min(count, beg + tile);
+    for (uint32_t t = beg + threadIdx.x; t < end; t += SORT_THREADS) {
+        Fr s = load_scalar(scalars, list ? list[t] : t);
+        for_each_digit(s, D, [&](int j, uint32_t b, bool) { atomicAdd(&s_bin[((uint32_t)j * D.window_bucket_stride + b) >> fine_bits], 1u); });
+    }
+    __syncthreads();
+    for (uint32_t i = threadIdx.x; i < n_parts; i += SORT_THREADS) mat[(size_t)i * gridDim.x + blockIdx.x] = s_bin[i];
+}
+
+// off = the scanned coarse matrix.  The block recomputes the digits of the count pass (tile * n_windows <= SORT_STAGE),
+// sorts them by partition in shared memory and stores each partition's run at off[part][block] in stage / stage_fine.
+static __global__ void __launch_bounds__(SORT_THREADS)
+sort_coarse_scatter_kernel(const uint8_t* __restrict__ scalars, const uint32_t* __restrict__ list, const uint32_t* __restrict__ count_ptr,
+                           uint32_t count_fixed, Digits D, int fine_bits, uint32_t n_parts, uint32_t tile, const uint32_t* __restrict__ off,
+                           uint32_t* __restrict__ stage, uint16_t* __restrict__ stage_fine) {
+    __shared__ uint32_t s_base[SORT_PARTS + 1], s_cur[SORT_PARTS], s_goff[SORT_PARTS], s_tmp[SORT_THREADS];
+    __shared__ uint32_t s_word[SORT_STAGE];
+    __shared__ uint16_t s_fine[SORT_STAGE];
+    const uint32_t count = count_ptr ? *count_ptr : count_fixed;
+    for (uint32_t p = threadIdx.x; p < SORT_PARTS; p += SORT_THREADS) {
+        const size_t c = (size_t)p * gridDim.x + blockIdx.x;      // the next cell in scan order holds the next offset
+        s_goff[p] = p < n_parts ? off[c] : 0;
+        s_base[p] = p < n_parts ? off[c + 1] - off[c] : 0;
+    }
+    __syncthreads();
+    block_exclusive_scan<SORT_THREADS>(s_base, SORT_PARTS, s_tmp);
+    for (uint32_t p = threadIdx.x; p < SORT_PARTS; p += SORT_THREADS) s_cur[p] = s_base[p];
+    __syncthreads();
+    const uint32_t beg = blockIdx.x * tile, end = min(count, beg + tile);
+    for (uint32_t t = beg + threadIdx.x; t < end; t += SORT_THREADS) {
+        const uint32_t idx = list ? list[t] : t;
+        Fr s = load_scalar(scalars, idx);
+        for_each_digit(s, D, [&](int j, uint32_t b, bool neg) {
+            const uint32_t bucket = (uint32_t)j * D.window_bucket_stride + b;
+            const uint32_t pos = atomicAdd(&s_cur[bucket >> fine_bits], 1u);
+            s_word[pos] = ((uint32_t)j * D.window_point_stride + idx) | (neg ? 0x80000000u : 0u);
+            s_fine[pos] = (uint16_t)(bucket & ((1u << fine_bits) - 1));
+        });
+    }
+    __syncthreads();
+    for (uint32_t i = threadIdx.x; i < s_base[SORT_PARTS]; i += SORT_THREADS) {
+        const uint32_t p = sort_tile_part(s_base, SORT_PARTS, i);
+        const uint32_t g = s_goff[p] + (i - s_base[p]);
+        stage[g] = s_word[i];
+        stage_fine[g] = s_fine[i];
+    }
+}
+
+// part_count[p] = digits of partition p (from the scanned coarse matrix)
+static __global__ void sort_part_count_kernel(const uint32_t* __restrict__ coarse_off, uint32_t coarse_blocks, uint32_t n_parts,
+                                              uint32_t* part_count) {
+    const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
+    if (p < n_parts) part_count[p] = coarse_off[(size_t)(p + 1) * coarse_blocks] - coarse_off[(size_t)p * coarse_blocks];
+}
+
+// the staged digits [beg, end) of fine tile w (block w of the fine passes); false past the last tile
+__device__ __forceinline__ bool sort_fine_tile(const uint32_t* coarse_off, uint32_t coarse_blocks, const uint32_t* tile_base, uint32_t n_parts,
+                                               uint32_t w, uint32_t& tb, uint32_t& tiles_p, uint32_t& t, uint32_t& beg, uint32_t& end) {
+    if (w >= tile_base[n_parts]) return false;
+    const uint32_t p = sort_tile_part(tile_base, n_parts, w);
+    tb = tile_base[p]; tiles_p = tile_base[p + 1] - tb; t = w - tb;
+    beg = coarse_off[(size_t)p * coarse_blocks] + t * SORT_TILE;
+    end = min(coarse_off[(size_t)(p + 1) * coarse_blocks], beg + SORT_TILE);
+    return true;
+}
+
+// counts fine tile w's digits per fine bin into mat; blocks past the last tile zero their cells, so that the host can
+// scan gridDim.x << fine_bits cells
+static __global__ void __launch_bounds__(SORT_THREADS)
+sort_fine_count_kernel(const uint32_t* __restrict__ coarse_off, uint32_t coarse_blocks, const uint32_t* __restrict__ tile_base,
+                       uint32_t n_parts, int fine_bits, const uint16_t* __restrict__ stage_fine, uint32_t* mat) {
+    __shared__ uint32_t s_bin[1u << SORT_MAX_FINE_BITS];
+    const uint32_t n_fine = 1u << fine_bits;
+    uint32_t tb, tiles_p, t, beg, end;
+    if (!sort_fine_tile(coarse_off, coarse_blocks, tile_base, n_parts, blockIdx.x, tb, tiles_p, t, beg, end)) {
+        for (uint32_t f = threadIdx.x; f < n_fine; f += SORT_THREADS) mat[((size_t)blockIdx.x << fine_bits) + f] = 0;
+        return;
+    }
+    for (uint32_t f = threadIdx.x; f < n_fine; f += SORT_THREADS) s_bin[f] = 0;
+    __syncthreads();
+    for (uint32_t k = beg + threadIdx.x; k < end; k += SORT_THREADS) atomicAdd(&s_bin[stage_fine[k]], 1u);
+    __syncthreads();
+    for (uint32_t f = threadIdx.x; f < n_fine; f += SORT_THREADS) mat[sort_cell(tb, tiles_p, f, t, fine_bits)] = s_bin[f];
+}
+
+// off = the scanned fine matrix.  Sorts fine tile w by bucket in shared memory (SORT_FINE_SMEM bytes) and stores each
+// bucket's run at its offset in entries.
+static __global__ void __launch_bounds__(SORT_FINE_THREADS)
+sort_fine_scatter_kernel(const uint32_t* __restrict__ coarse_off, uint32_t coarse_blocks, const uint32_t* __restrict__ tile_base,
+                         uint32_t n_parts, int fine_bits, const uint32_t* __restrict__ stage, const uint16_t* __restrict__ stage_fine,
+                         const uint32_t* __restrict__ off, uint32_t* __restrict__ entries) {
+    extern __shared__ uint32_t smem[];
+    const uint32_t n_fine = 1u << fine_bits;
+    uint32_t* s_base = smem;                     // n_fine + 1
+    uint32_t* s_cur = s_base + n_fine + 1;       // n_fine
+    uint32_t* s_goff = s_cur + n_fine;           // n_fine
+    uint32_t* s_tmp = s_goff + n_fine;           // SORT_FINE_THREADS
+    uint32_t* s_word = s_tmp + SORT_FINE_THREADS;   // SORT_TILE
+    uint32_t tb, tiles_p, t, beg, end;
+    if (!sort_fine_tile(coarse_off, coarse_blocks, tile_base, n_parts, blockIdx.x, tb, tiles_p, t, beg, end)) return;
+    for (uint32_t f = threadIdx.x; f < n_fine; f += SORT_FINE_THREADS) {
+        const size_t c = sort_cell(tb, tiles_p, f, t, fine_bits);   // the next cell in scan order holds the next offset
+        s_goff[f] = off[c];
+        s_base[f] = off[c + 1] - off[c];
+    }
+    __syncthreads();
+    block_exclusive_scan<SORT_FINE_THREADS>(s_base, n_fine, s_tmp);
+    for (uint32_t f = threadIdx.x; f < n_fine; f += SORT_FINE_THREADS) s_cur[f] = s_base[f];
+    __syncthreads();
+    for (uint32_t k = beg + threadIdx.x; k < end; k += SORT_FINE_THREADS) s_word[atomicAdd(&s_cur[stage_fine[k]], 1u)] = stage[k];
+    __syncthreads();
+    for (uint32_t i = threadIdx.x; i < end - beg; i += SORT_FINE_THREADS) {
+        const uint32_t f = sort_tile_part(s_base, n_fine, i);
+        entries[s_goff[f] + (i - s_base[f])] = s_word[i];
+    }
+}
+
+// offsets[b] for b in [0, n_buckets], hist[b] = offsets[b + 1] - offsets[b] (hist[n_buckets] = 0)
+static __global__ void sort_offsets_kernel(uint32_t n_buckets, int fine_bits, const uint32_t* __restrict__ coarse_off, uint32_t coarse_blocks,
+                                           const uint32_t* __restrict__ tile_base, const uint32_t* __restrict__ fine_off,
+                                           uint32_t* hist, uint32_t* offsets) {
+    const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b > n_buckets) return;
+    const uint32_t o = sort_bucket_offset(b, n_buckets, fine_bits, coarse_off, coarse_blocks, tile_base, fine_off);
+    offsets[b] = o;
+    hist[b] = b < n_buckets ? sort_bucket_offset(b + 1, n_buckets, fine_bits, coarse_off, coarse_blocks, tile_base, fine_off) - o : 0;
+}
+
+// one-level counting sort (small bucket sets): global histogram, its exclusive scan, scatter with a cursor per bucket
 static __global__ void digit_hist_kernel(const uint8_t* __restrict__ scalars, const uint32_t* __restrict__ list,
-                                  const uint32_t* __restrict__ count_ptr, uint32_t count_fixed, Digits D, uint32_t* hist) {
+                                         const uint32_t* __restrict__ count_ptr, uint32_t count_fixed, Digits D, uint32_t* hist) {
     const uint32_t count = count_ptr ? *count_ptr : count_fixed;
     for (uint32_t t = blockIdx.x * blockDim.x + threadIdx.x; t < count; t += gridDim.x * blockDim.x) {
         const uint32_t idx = list ? list[t] : t;
@@ -151,10 +331,9 @@ static __global__ void digit_hist_kernel(const uint8_t* __restrict__ scalars, co
         for_each_digit(s, D, [&](int j, uint32_t b, bool) { atomicAdd(&hist[(uint32_t)j * D.window_bucket_stride + b], 1u); });
     }
 }
-
 static __global__ void digit_scatter_kernel(const uint8_t* __restrict__ scalars, const uint32_t* __restrict__ list,
-                                     const uint32_t* __restrict__ count_ptr, uint32_t count_fixed, Digits D,
-                                     const uint32_t* __restrict__ offsets, uint32_t* cursor, uint32_t* entries) {
+                                            const uint32_t* __restrict__ count_ptr, uint32_t count_fixed, Digits D,
+                                            const uint32_t* __restrict__ offsets, uint32_t* cursor, uint32_t* entries) {
     const uint32_t count = count_ptr ? *count_ptr : count_fixed;
     for (uint32_t t = blockIdx.x * blockDim.x + threadIdx.x; t < count; t += gridDim.x * blockDim.x) {
         const uint32_t idx = list ? list[t] : t;
@@ -166,22 +345,18 @@ static __global__ void digit_scatter_kernel(const uint8_t* __restrict__ scalars,
         });
     }
 }
-// The same counting-sort scatter, moving the POINTS instead of their indices (batched-affine path): thread t reads
-// point t of every table level - consecutive threads read consecutive points, so the 3.5 GB table streams in coalesced
-// - and writes the (sign-adjusted) point to its place in bucket order.  The sweeps then work on flat arrays only.
+
+// the batched-affine path works on the points themselves: sorted[k] = the (sign-adjusted) point of entry k
 template <class F>
 __global__ void __launch_bounds__(256)
-digit_scatter_points_kernel(const uint8_t* __restrict__ scalars, uint32_t count, Digits D, const uint32_t* __restrict__ offsets,
-                            uint32_t* cursor, const uint8_t* __restrict__ points, Affine<F>* __restrict__ sorted) {
-    for (uint32_t idx = blockIdx.x * blockDim.x + threadIdx.x; idx < count; idx += gridDim.x * blockDim.x) {
-        Fr s = load_scalar(scalars, idx);
-        for_each_digit(s, D, [&](int j, uint32_t b, bool neg) {
-            const uint32_t bucket = (uint32_t)j * D.window_bucket_stride + b;
-            const uint32_t pos = offsets[bucket] + atomicAdd(&cursor[bucket], 1u);
-            Affine<F> p = Affine<F>::load(points + sizeof(Affine<F>) * ((size_t)j * D.window_point_stride + idx));
-            if (neg) p.y = p.y.neg();
-            p.store(sorted + pos);
-        });
+gather_points_kernel(const uint32_t* __restrict__ entries, const uint32_t* __restrict__ offsets, uint32_t n_buckets,
+                     const uint8_t* __restrict__ points, Affine<F>* __restrict__ sorted) {
+    const uint32_t total = offsets[n_buckets];
+    for (uint32_t k = blockIdx.x * blockDim.x + threadIdx.x; k < total; k += gridDim.x * blockDim.x) {
+        const uint32_t e = entries[k];
+        Affine<F> p = Affine<F>::load(points + sizeof(Affine<F>) * (size_t)(e & 0x7fffffffu));
+        if (e >> 31) p.y = p.y.neg();
+        p.store(sorted + k);
     }
 }
 
@@ -256,6 +431,52 @@ static void exclusive_scan(const uint32_t* in, uint32_t n, uint32_t chunk, uint3
     scan_tile_apply_kernel<<<n_tiles, 256, 0, st>>>(in, n, chunk, levels, tiles, out);
     ZKE_COUNT_LAUNCH(3);
 }
+
+// ---------------------------------------------------------------- bucket sort: workspace and launches
+struct DigitSort {
+    uint32_t n_buckets, n_parts, coarse_tile, coarse_blocks, fine_blocks;
+    int fine_bits = 0;
+    size_t max_entries, coarse_cells, fine_cells;
+    uint32_t *coarse, *coarse_off, *part_count, *tile_base, *fine, *fine_off, *tiles, *stage;
+    uint16_t* stage_fine;
+    DigitSort(uint32_t n, int n_windows, uint32_t n_buckets_, size_t max_entries_) : n_buckets(n_buckets_), max_entries(max_entries_) {
+        while ((n_buckets - 1) >> fine_bits >= SORT_PARTS) ++fine_bits;      // at most SORT_PARTS partitions
+        n_parts = sort_parts(n_buckets, fine_bits);
+        coarse_tile = SORT_STAGE / (uint32_t)n_windows;      // a scalar has at most n_windows digits
+        coarse_blocks = std::max(1u, (n + coarse_tile - 1) / coarse_tile);
+        fine_blocks = (uint32_t)(max_entries / SORT_TILE + n_parts);    // >= sum over partitions of ceil(size / SORT_TILE)
+        coarse_cells = (size_t)n_parts * coarse_blocks;
+        fine_cells = (size_t)fine_blocks << fine_bits;
+    }
+    // carves the sort's arrays out of the workspace through take(bytes)
+    template <class Take> void place(Take take) {
+        coarse = (uint32_t*)take(4 * (coarse_cells + 1));
+        coarse_off = (uint32_t*)take(4 * (coarse_cells + 1));
+        part_count = (uint32_t*)take(4 * ((size_t)n_parts + 1));
+        tile_base = (uint32_t*)take(4 * ((size_t)n_parts + 1));
+        fine = (uint32_t*)take(4 * (fine_cells + 1));
+        fine_off = (uint32_t*)take(4 * (fine_cells + 1));
+        tiles = (uint32_t*)take(4 * (std::max(coarse_cells, fine_cells) / SCAN_TILE + 2));
+        stage = (uint32_t*)take(4 * max_entries);
+        stage_fine = (uint16_t*)take(2 * max_entries);
+    }
+    // hist / offsets / entries (layout above) of the digits of scalars[list[0 .. *count_ptr)] (list == nullptr:
+    // scalars[0 .. count_fixed)); count_fixed is also the upper bound of *count_ptr
+    void run(const uint8_t* scalars, const uint32_t* list, const uint32_t* count_ptr, uint32_t count_fixed, const Digits& D,
+             uint32_t* hist, uint32_t* offsets, uint32_t* entries, cudaStream_t st) const {
+        sort_coarse_count_kernel<<<coarse_blocks, SORT_THREADS, 0, st>>>(scalars, list, count_ptr, count_fixed, D, fine_bits, n_parts, coarse_tile, coarse);
+        exclusive_scan(coarse, (uint32_t)coarse_cells, 0, 0, coarse_off, tiles, st);
+        sort_coarse_scatter_kernel<<<coarse_blocks, SORT_THREADS, 0, st>>>(scalars, list, count_ptr, count_fixed, D, fine_bits, n_parts, coarse_tile, coarse_off, stage, stage_fine);
+        sort_part_count_kernel<<<(n_parts + 255) / 256, 256, 0, st>>>(coarse_off, coarse_blocks, n_parts, part_count);
+        exclusive_scan(part_count, n_parts, SORT_TILE, 0, tile_base, tiles, st);
+        sort_fine_count_kernel<<<fine_blocks, SORT_THREADS, 0, st>>>(coarse_off, coarse_blocks, tile_base, n_parts, fine_bits, stage_fine, fine);
+        exclusive_scan(fine, (uint32_t)fine_cells, 0, 0, fine_off, tiles, st);
+        cudaFuncSetAttribute(sort_fine_scatter_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SORT_FINE_SMEM);
+        sort_fine_scatter_kernel<<<fine_blocks, SORT_FINE_THREADS, SORT_FINE_SMEM, st>>>(coarse_off, coarse_blocks, tile_base, n_parts, fine_bits, stage, stage_fine, fine_off, entries);
+        sort_offsets_kernel<<<(n_buckets + 256) / 256, 256, 0, st>>>(n_buckets, fine_bits, coarse_off, coarse_blocks, tile_base, fine_off, hist, offsets);
+        ZKE_COUNT_LAUNCH(6);
+    }
+};
 
 static __global__ void fill_work_kernel(const uint32_t* __restrict__ hist, const uint32_t* __restrict__ chunk_off, uint32_t n_buckets,
                                  uint32_t CHUNK, uint32_t levels, uint32_t* work_bucket) {
@@ -536,7 +757,6 @@ size_t MsmPlan<F>::workspace_bytes(uint32_t n, const MsmConfig& cfg) {
     al(4 * (size_t)n);                 // general list
     al(4 * (n_buckets + 1));           // hist
     al(4 * (n_buckets + 1));           // offsets
-    al(4 * (n_buckets + 1));           // cursor
     al(4 * (n_buckets + 1));           // chunk_off
     al(4 * (n_buckets / SCAN_TILE + 2));  // scan tiles
     al(4 * max_entries);               // entries
@@ -552,6 +772,8 @@ size_t MsmPlan<F>::workspace_bytes(uint32_t n, const MsmConfig& cfg) {
     al(4 * (order_cells + 1));                // per-block size histograms, bin-major
     al(4 * (order_cells + 1));                // their exclusive scan
     al(4 * (order_cells / SCAN_TILE + 2));    // scan tiles
+    if (n_buckets >= SORT_TWO_LEVEL_MIN_BUCKETS) DigitSort((uint32_t)n, W, (uint32_t)n_buckets, max_entries).place([&](size_t x) { al(x); return (uint8_t*)nullptr; });
+    else al(4 * (n_buckets + 1));             // cursor
     return b;
 }
 
@@ -580,7 +802,6 @@ void MsmPlan<F>::run(const uint8_t* points, const uint8_t* scalars, uint32_t n, 
     uint32_t* gen_list = (uint32_t*)take(4 * (size_t)n);
     uint32_t* hist = (uint32_t*)take(4 * ((size_t)n_buckets + 1));
     uint32_t* offsets = (uint32_t*)take(4 * ((size_t)n_buckets + 1));
-    uint32_t* cursor = (uint32_t*)take(4 * ((size_t)n_buckets + 1));
     uint32_t* chunk_off = (uint32_t*)take(4 * ((size_t)n_buckets + 1));
     uint32_t* tiles = (uint32_t*)take(4 * ((size_t)n_buckets / SCAN_TILE + 2));
     uint32_t* entries = (uint32_t*)take(4 * max_entries);
@@ -599,6 +820,12 @@ void MsmPlan<F>::run(const uint8_t* points, const uint8_t* scalars, uint32_t n, 
     uint32_t* order_mat = (uint32_t*)take(4 * (order_cells + 1));
     uint32_t* order_off = (uint32_t*)take(4 * (order_cells + 1));
     uint32_t* order_tiles = (uint32_t*)take(4 * (order_cells / SCAN_TILE + 2));
+    const bool two_level = n_buckets >= SORT_TWO_LEVEL_MIN_BUCKETS;
+    DigitSort sort(n, D.n_windows, n_buckets, max_entries);
+    if (sort.fine_bits > SORT_MAX_FINE_BITS) throw std::runtime_error("MSM bucket sort: more than 2^19 buckets");
+    uint32_t* cursor = nullptr;
+    if (two_level) sort.place(take);
+    else cursor = (uint32_t*)take(4 * ((size_t)n_buckets + 1));
 
     // result block: [MSM_ONES_SLOTS partial sums of the unit-scalar points][MSM_MAX_WINDOWS window sums]
     uint8_t* res_ones = result;
@@ -632,15 +859,20 @@ void MsmPlan<F>::run(const uint8_t* points, const uint8_t* scalars, uint32_t n, 
         gen_count = counters + 1;
         gen_idx = gen_list;
     }
-    cudaMemsetAsync(hist, 0, 4 * ((size_t)n_buckets + 1), st);
-    cudaMemsetAsync(cursor, 0, 4 * ((size_t)n_buckets + 1), st);
     const int sms = sm_count();
-    const int grid = sms * 8;
-    digit_hist_kernel<<<grid, 256, 0, st>>>(scalars, gen_idx, gen_count, n, D, hist);
-    exclusive_scan(hist, n_buckets, 0, 0, offsets, tiles, st);
-    if (use_ba) digit_scatter_points_kernel<F><<<grid, 256, 0, st>>>(scalars, n, D, offsets, cursor, points, (Affine<F>*)ba_ws);
-    else digit_scatter_kernel<<<grid, 256, 0, st>>>(scalars, gen_idx, gen_count, n, D, offsets, cursor, entries);
+    if (two_level) {
+        sort.run(scalars, gen_idx, gen_count, n, D, hist, offsets, entries, st);
+    } else {
+        cudaMemsetAsync(hist, 0, 4 * ((size_t)n_buckets + 1), st);
+        cudaMemsetAsync(cursor, 0, 4 * ((size_t)n_buckets + 1), st);
+        digit_hist_kernel<<<sms * 8, 256, 0, st>>>(scalars, gen_idx, gen_count, n, D, hist);
+        exclusive_scan(hist, n_buckets, 0, 0, offsets, tiles, st);
+        digit_scatter_kernel<<<sms * 8, 256, 0, st>>>(scalars, gen_idx, gen_count, n, D, offsets, cursor, entries);
+        ZKE_COUNT_LAUNCH(2);
+    }
     if (use_ba) {
+        gather_points_kernel<F><<<sms * 8, 256, 0, st>>>(entries, offsets, n_buckets, points, (Affine<F>*)ba_ws);
+        ZKE_COUNT_LAUNCH(1);
         run_ba<F>(cfg, hist, offsets, n_buckets, max_entries, tiles, ba_ws, D, groups, group_out, st, ev, heavy);
     } else {
         exclusive_scan(hist, n_buckets, D.chunk, 0, chunk_off, tiles, st);
@@ -713,7 +945,7 @@ void MsmPlan<F>::run(const uint8_t* points, const uint8_t* scalars, uint32_t n, 
     }
     window_reduce_kernel<F><<<bucket_sets, 512, 0, st>>>(group_out, groups_per_window);
     gather_windows_kernel<F><<<1, 64, 0, st>>>(group_out, groups_per_window, bucket_sets, res_windows);
-    ZKE_COUNT_LAUNCH(7);
+    ZKE_COUNT_LAUNCH(5);
 }
 
 #if defined(ZKE_MSM_G1)
