@@ -239,6 +239,27 @@ int zke_verify_json(const char* vkey_json, const char* public_json, const char* 
  * by one to name the offenders.  Returns the number of valid proofs, < 0 on malformed input.  Host only. */
 int zke_verify_batch_json(const char* vkey_json, const char* publics_json, const char* proofs_json, const uint8_t* rand16,
                           uint8_t* ok, char* err, size_t errcap);
+/* ---------------------------------------------------------------------------------------------------
+ * Batch verification on the GPU: snarkjs.groth16.verify(vkey, publicSignals, proof)
+ * (/root/reference/packages/helpers/src/chunked-zkey.ts:101) for n proofs under one key per call, with the verdicts of
+ * zke_verify_batch_json.  The proofs are validated in parallel (coordinates below q, points on their curves, B in the
+ * order-r subgroup, n_public signals below r); then ONE randomised product of n + 3 Miller loops and one final
+ * exponentiation checks them all; if a proof is malformed or that check fails, every proof is verified on its own.
+ * ------------------------------------------------------------------------------------------------- */
+typedef struct zke_verifier zke_verifier;
+/* vkey.json in; validates the key (points on their curves, G2 points in the subgroup), precomputes the Miller-loop lines
+ * of beta_2, gamma_2, delta_2 and e(alpha, beta), and keeps them on GPU `device`.  NULL + message for an invalid key. */
+zke_verifier* zke_verifier_open(const char* vkey_json, int device, char* err, size_t errcap);
+void zke_verifier_close(zke_verifier* v);
+/* proofs: [n][8][32] in zke_prove's layout (an all-zero point is the point at infinity); publics: [n][n_public][32]
+ * (n_public = number of IC points - 1), standard form LE; rand16: n x 16 bytes of caller randomness the provers cannot
+ * predict, or NULL (/dev/urandom); a zero weight counts as 1.  ok (may be NULL): ok[i] = 1 / 0.
+ * Returns the number of valid proofs, < 0 on a fatal error. */
+int zke_verifier_batch(zke_verifier* v, size_t n, const uint8_t* proofs, const uint8_t* publics, const uint8_t* rand16,
+                       uint8_t* ok, char* err, size_t errcap);
+/* Diagnostic: e(P_i, Q_i) for n pairs on GPU `device`, in zke_pairing_alphabeta's output layout (g1: [n][64],
+ * g2: [n][128], out: [n][384]; standard form LE).  Points must be on their curves (< 0 otherwise). */
+int zke_selftest_pairing_gpu(int device, size_t n, const uint8_t* g1, const uint8_t* g2, uint8_t* out, char* err, size_t errcap);
 /* `snarkjs zkey export verificationkey`, incl. vk_alphabeta_12 = e(alpha_1, beta_2) in snarkjs' Fq12 tower layout
  * (/root/reference/packages/rust-verifier/tests/data/proof_of_twitter/vkey.json:43). */
 int zke_zkey_vkey_json(const zke_zkey* z, char* out, size_t* len);

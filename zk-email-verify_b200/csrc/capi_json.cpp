@@ -176,6 +176,20 @@ void flatten_values(const JV& v, std::vector<U256>& out) {
 
 }  // namespace
 
+VerifyingKey zke::vkey_from_json(const char* json) {
+    JV vk = JParser(json).parse();
+    const JV* prot = vk.get("protocol");
+    if (prot && prot->s != "groth16") throw std::runtime_error("vkey protocol is not groth16");
+    VerifyingKey k;
+    k.alpha1 = g1_of(need(vk, "vk_alpha_1"));
+    k.beta2 = g2_of(need(vk, "vk_beta_2"));
+    k.gamma2 = g2_of(need(vk, "vk_gamma_2"));
+    k.delta2 = g2_of(need(vk, "vk_delta_2"));
+    for (auto& p : need(vk, "IC").arr) k.ic.push_back(g1_of(p));
+    if (k.ic.empty()) throw std::runtime_error("vkey has no IC");
+    return k;
+}
+
 extern "C" {
 
 int zke_verify_json(const char* vkey_json, const char* public_json, const char* proof_json, char* err, size_t errcap) {

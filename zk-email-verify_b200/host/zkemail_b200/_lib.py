@@ -84,6 +84,10 @@ zke_prove = _sig("zke_prove", c_int, [c_void_p, c_size_t, c_void_p, c_void_p, c_
 zke_fullprove = _sig("zke_fullprove", c_int, [c_void_p, c_void_p, c_size_t, c_void_p, c_void_p, c_void_p, c_void_p, c_char_p, c_size_t])
 zke_verify_json = _sig("zke_verify_json", c_int, [c_char_p, c_char_p, c_char_p, c_char_p, c_size_t])
 zke_verify_batch_json = _sig("zke_verify_batch_json", c_int, [c_char_p, c_char_p, c_char_p, c_void_p, c_void_p, c_char_p, c_size_t])
+zke_verifier_open = _sig("zke_verifier_open", c_void_p, [c_char_p, c_int, c_char_p, c_size_t])
+zke_verifier_close = _sig("zke_verifier_close", None, [c_void_p])
+zke_verifier_batch = _sig("zke_verifier_batch", c_int, [c_void_p, c_size_t, c_void_p, c_void_p, c_void_p, c_void_p, c_char_p, c_size_t])
+zke_selftest_pairing_gpu = _sig("zke_selftest_pairing_gpu", c_int, [c_int, c_size_t, c_void_p, c_void_p, c_void_p, c_char_p, c_size_t])
 zke_zkey_vkey_json = _sig("zke_zkey_vkey_json", c_int, [c_void_p, c_char_p, ctypes.POINTER(c_size_t)])
 zke_proof_to_json = _sig("zke_proof_to_json", c_int, [c_void_p, c_void_p, c_u32, c_char_p, ctypes.POINTER(c_size_t), c_char_p, ctypes.POINTER(c_size_t)])
 zke_pack_inputs_json = _sig("zke_pack_inputs_json", c_int, [c_void_p, c_char_p, c_void_p, c_size_t, c_char_p, c_size_t])
