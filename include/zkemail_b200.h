@@ -134,6 +134,34 @@ enum {
 int64_t zke_zkey_section(const zke_zkey* z, int section, uint8_t* out, size_t cap);
 
 /* ---------------------------------------------------------------------------------------------------
+ * Keys from a Powers-of-Tau file (`snarkjs groth16 setup` / `zkey new`, then `zkey contribute`; the route of
+ * /root/reference/docs/zk-email-docs/UsageGuide/README.md:149-180), for this engine's own R1CS.
+ * ------------------------------------------------------------------------------------------------- */
+/* A prepared phase-2 `.ptau` image (layout in setup.cu) -> key with gamma = delta = 1 on GPU `device`: the sums of
+ * Lagrange-basis points of every signal, computed on the GPU.  The file must hold the Lagrange bases of size 2^(domain_log2 + 1);
+ * every point used is validated.  Such a key reports zke_zkey_is_toy = 1 (anyone can forge proofs while delta = 1) until
+ * zke_zkey_contribute is applied. */
+zke_zkey* zke_zkey_from_ptau(const zke_circuit* c, const void* ptau, size_t len, int device, char* err, size_t errcap);
+/* Host-only structure check of a `.ptau` image (magic, modulus, every section size against its power and, with c != NULL,
+ * that it is large enough for c): power, and per section type < 16 its payload offset and size in the file (0 if absent). */
+int zke_ptau_info(const zke_circuit* c, const void* ptau, size_t len, uint32_t* power, uint64_t* offsets16, uint64_t* sizes16,
+                  char* err, size_t errcap);
+/* Wall time of this thread's last zke_zkey_from_ptau: host part (parse, transpose) and device part (upload, sums, H table). */
+int zke_zkey_from_ptau_timing(double* host_ms, double* gpu_ms);
+/* Phase-2 contribution with secret s (32 bytes LE, 1 < s < r): a NEW key with delta1, delta2 times s and the C ("L") and H
+ * points times s^-1; everything else copied.  Not a snarkjs transcript: the result can be contributed to again here, not by
+ * snarkjs.  A contribution to a zke_zkey_from_ptau key makes it a real key (is_toy 0); one to a zke_setup key stays a toy. */
+zke_zkey* zke_zkey_contribute(const zke_zkey* prev, const uint8_t* secret32, char* err, size_t errcap);
+/* The ratio check of `snarkjs zkey verify`: 1 if `next` follows from `prev` by contributions (header, IC, A, B1, B2 and the
+ * coefficient matrices identical; e(delta1', G2) == e(G1, delta2'); e(X', delta2') == e(X, delta2) for X a random 128-bit
+ * combination of the L and H points, weights derived from rand16, or /dev/urandom when NULL), 0 if not with the reason in
+ * err, < 0 on errors.  Both keys must live on one device. */
+int zke_zkey_check_contribution(const zke_zkey* prev, const zke_zkey* next, const uint8_t* rand16, char* err, size_t errcap);
+/* TOY prepared `.ptau` image from KNOWN tau, alpha, beta (3 x 32 bytes LE, in [1, r)) - tests and measurement only, like
+ * zke_setup.  out == NULL: returns the size needed; -2 if cap is too small; < 0 on error. */
+int64_t zke_ptau_toy(uint32_t power, const uint8_t* tau_alpha_beta96, int device, uint8_t* out, size_t cap, char* err, size_t errcap);
+
+/* ---------------------------------------------------------------------------------------------------
  * Contexts: circuit (+ optional proving key) resident on one GPU with work buffers for `max_batch` emails.
  * One host thread per context (or external locking).  All calls are synchronous at the ABI.
  * ------------------------------------------------------------------------------------------------- */

@@ -150,6 +150,8 @@ bool groth16_verify(const VerifyingKey& vk, const std::vector<U256>& publics, co
 bool groth16_verify_batch(const VerifyingKey& vk, const std::vector<std::vector<U256>>& publics, const std::vector<Proof>& proofs,
                           const std::vector<U256>& rnd);
 bool g2_in_subgroup(const G2AffineH& p);
+// prod_i e(P_i, Q_i) == 1 (points on their curves, G2 points in the subgroup)
+bool pairing_product_is_one(const std::vector<std::pair<G1AffineH, G2AffineH>>& terms);
 // snarkjs vkey.json -> key (capi_json.cpp); throws on malformed JSON, unreduced coordinates or an empty IC
 VerifyingKey vkey_from_json(const char* json);
 void pairing_alphabeta(const G1AffineH& alpha1, const G2AffineH& beta2, U256 out[12]);   // snarkjs vk_alphabeta_12, [i][j][k] flattened

@@ -139,7 +139,8 @@ std::vector<U256> to_standard(const std::vector<Fr>& v) {
 struct zke_zkey {
     uint32_t n_vars = 0, n_public = 0, log_n = 0;
     int device = 0;
-    bool toy = false;         // made by zke_setup: the toxic waste is known
+    bool toy = false;         // made by zke_setup (the toxic waste is known) or by zke_zkey_from_ptau (delta = 1)
+    bool delta_one = false;   // made by zke_zkey_from_ptau and not yet contributed to: toy until a contribution
     G1AffineH alpha1, beta1, delta1;
     G2AffineH beta2, gamma2, delta2;
     std::vector<G1AffineH> ic;
@@ -370,18 +371,22 @@ __global__ void validate_points_kernel(const uint8_t* __restrict__ pts, uint32_t
 }
 
 template <class F, class HostF>
-void validate_points(const DevBuf& buf, size_t n, const HostF& b_host, const char* what, uint32_t* flag_dev) {
+void validate_points(const uint8_t* pts, size_t n, const HostF& b_host, const char* what, uint32_t* flag_dev, const char* file = ".zkey") {
     if (!n) return;
     F b;
     static_assert(sizeof(F) == sizeof(HostF), "host / device field images differ");
     memcpy(&b, &b_host, sizeof(F));
     CUDA_OK(cudaMemset(flag_dev, 0xff, 4));
-    validate_points_kernel<F><<<(unsigned)((n + 127) / 128), 128>>>(buf.p, (uint32_t)n, b, flag_dev);
+    validate_points_kernel<F><<<(unsigned)((n + 127) / 128), 128>>>(pts, (uint32_t)n, b, flag_dev);
     ZKE_COUNT_LAUNCH(1);
     CHECK_LAUNCH();
     uint32_t bad = 0;
     CUDA_OK(cudaMemcpy(&bad, flag_dev, 4, cudaMemcpyDeviceToHost));
-    if (bad != 0xffffffffu) throw std::runtime_error(std::string(".zkey section ") + what + ": point " + std::to_string(bad) + " is not on the curve");
+    if (bad != 0xffffffffu) throw std::runtime_error(std::string(file) + " section " + what + ": point " + std::to_string(bad) + " is not on the curve");
+}
+template <class F, class HostF>
+void validate_points(const DevBuf& buf, size_t n, const HostF& b_host, const char* what, uint32_t* flag_dev) {
+    validate_points<F>(buf.p, n, b_host, what, flag_dev);
 }
 
 Fq2 g2_twist_b() { return Fq2{Fq::from_u64(3), Fq::zero()} * Fq2{Fq::from_u64(9), Fq::one()}.inv(); }
@@ -1748,3 +1753,7 @@ int zke_shard_combine_raw(const uint8_t* key_points, const uint8_t* partials, in
 }
 
 }  // extern "C"
+
+// Key construction from a Powers-of-Tau file, phase-2 contributions and their check: part of this translation unit,
+// because it builds zke_zkey objects the same way do_setup / do_zkey_load do.
+#include "setup.cu"

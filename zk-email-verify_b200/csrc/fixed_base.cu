@@ -85,6 +85,16 @@ void fixed_base_batch(const uint8_t* table, const uint8_t* scalars, uint32_t n, 
 template void fixed_base_batch<Fq>(const uint8_t*, const uint8_t*, uint32_t, uint8_t*, uint8_t*, cudaStream_t);
 template void fixed_base_batch<Fq2>(const uint8_t*, const uint8_t*, uint32_t, uint8_t*, uint8_t*, cudaStream_t);
 
+template <class F>
+void xyzz_to_affine_batch(const uint8_t* in_xyzz, uint32_t n, uint8_t* out_affine, cudaStream_t st) {
+    if (!n) return;
+    const uint32_t threads = (n + TO_AFFINE_BATCH - 1) / TO_AFFINE_BATCH;
+    xyzz_to_affine_kernel<F><<<(threads + 127) / 128, 128, 0, st>>>(in_xyzz, n, out_affine);
+    ZKE_COUNT_LAUNCH(1);
+}
+template void xyzz_to_affine_batch<Fq>(const uint8_t*, uint32_t, uint8_t*, cudaStream_t);
+template void xyzz_to_affine_batch<Fq2>(const uint8_t*, uint32_t, uint8_t*, cudaStream_t);
+
 }  // namespace dev
 }  // namespace zke
 

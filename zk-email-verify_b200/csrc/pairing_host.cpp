@@ -204,6 +204,12 @@ void pairing_alphabeta(const G1AffineH& alpha1, const G2AffineH& beta2, U256 out
         }
 }
 
+bool pairing_product_is_one(const std::vector<std::pair<G1AffineH, G2AffineH>>& terms) {
+    F12 f = F12::one();
+    for (auto& t : terms) f = mul(f, miller_loop(t.second, t.first));
+    return final_exponentiation(f) == F12::one();
+}
+
 bool groth16_verify(const VerifyingKey& vk, const std::vector<U256>& publics, const Proof& pr) {
     if (publics.size() + 1 != vk.ic.size()) return false;
     for (auto& s : publics) if (u256_cmp(s, fr_params().p) >= 0) return false;

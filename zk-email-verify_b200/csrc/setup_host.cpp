@@ -31,7 +31,7 @@ static Fr fr_from_seed(uint64_t seed, uint64_t stream) {
 void derive_toxic(uint64_t seed, Fr out[5]) { for (int i = 0; i < 5; ++i) out[i] = fr_from_seed(seed, (uint64_t)i + 1); }
 
 // out[i] = numer * omega^i / (x - omega^i) for i in [0, N)
-static void lagrange_like(const Fr& x, const Fr& numer, unsigned log_n, std::vector<Fr>& out) {
+void lagrange_like(const Fr& x, const Fr& numer, unsigned log_n, std::vector<Fr>& out) {
     const size_t N = (size_t)1 << log_n;
     out.resize(N);
     const Fr omega = fr_root_of_unity(log_n);

@@ -16,5 +16,8 @@ struct SetupScalars {
 SetupScalars compute_setup_scalars(const Circuit& c, uint64_t seed);
 // tau, alpha, beta, gamma, delta derived from the seed (the KNOWN toxic waste of the toy setup)
 void derive_toxic(uint64_t seed, Fr out[5]);
+// out[i] = numer * omega^i / (x - omega^i), i < 2^log_n, omega a primitive 2^log_n-th root; with numer = (x^N - 1) / N
+// these are the Lagrange basis polynomials of that domain evaluated at x.  x must not lie in the domain.
+void lagrange_like(const Fr& x, const Fr& numer, unsigned log_n, std::vector<Fr>& out);
 
 }  // namespace zke

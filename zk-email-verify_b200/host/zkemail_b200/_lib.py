@@ -99,7 +99,14 @@ zke_ctx_profile = _sig("zke_ctx_profile", c_int, [c_void_p, c_int])
 zke_ctx_profile_get = _sig("zke_ctx_profile_get", c_int, [c_void_p, ctypes.POINTER(ctypes.c_double), ctypes.POINTER(c_u64)])
 STAGES = ("witness", "matvec", "ntt", "msm_a", "msm_b1", "msm_c", "msm_h", "msm_h_buckets", "msm_b2")
 zke_setup_toxic = _sig("zke_setup_toxic", c_int, [c_u64, c_void_p])
-zke_selftest_fpmul_hint = _sig("zke_selftest_fpmul_hint", c_int, [c_u32, c_u32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p])
+zke_zkey_from_ptau = _sig("zke_zkey_from_ptau", c_void_p, [c_void_p, c_void_p, c_size_t, c_int, c_char_p, c_size_t])
+zke_ptau_info = _sig("zke_ptau_info", c_int, [c_void_p, c_void_p, c_size_t, ctypes.POINTER(c_u32), ctypes.POINTER(c_u64),
+                                              ctypes.POINTER(c_u64), c_char_p, c_size_t])
+zke_zkey_from_ptau_timing = _sig("zke_zkey_from_ptau_timing", c_int, [ctypes.POINTER(ctypes.c_double), ctypes.POINTER(ctypes.c_double)])
+zke_zkey_contribute = _sig("zke_zkey_contribute", c_void_p, [c_void_p, c_void_p, c_char_p, c_size_t])
+zke_zkey_check_contribution = _sig("zke_zkey_check_contribution", c_int, [c_void_p, c_void_p, c_void_p, c_char_p, c_size_t])
+zke_ptau_toy = _sig("zke_ptau_toy", c_i64, [c_u32, c_void_p, c_int, c_void_p, c_size_t, c_char_p, c_size_t])
+zke_selftest_fpmul_hint =_sig("zke_selftest_fpmul_hint", c_int, [c_u32, c_u32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p])
 
 (SEC_ALPHA1, SEC_BETA1, SEC_DELTA1, SEC_BETA2, SEC_GAMMA2, SEC_DELTA2) = (101, 102, 103, 104, 105, 106)
 (SEC_IC, SEC_A, SEC_B1, SEC_B2, SEC_C, SEC_H) = (3, 5, 6, 7, 8, 9)

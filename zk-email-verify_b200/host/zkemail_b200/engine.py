@@ -49,6 +49,46 @@ class Zkey:
             raise L.ZkeError(err.value.decode())
         return cls(circuit, device=device, _handle=h)
 
+    @classmethod
+    def from_ptau(cls, circuit: Circuit, ptau, device: int = 0):
+        """`snarkjs groth16 setup` for this engine's R1CS: a key from a prepared phase-2 `.ptau` (bytes, a writable buffer or
+        a path, which is memory-mapped).  gamma = delta = 1, so the key is a toy until `contribute` is applied."""
+        err = ctypes.create_string_buffer(L.ERRCAP)
+        with _ptau_buffer(ptau) as (ptr, n):
+            h = L.zke_zkey_from_ptau(circuit.handle, ptr, n, device, err, L.ERRCAP)
+        if not h:
+            raise L.ZkeError(err.value.decode())
+        return cls(circuit, device=device, _handle=h)
+
+    def contribute(self, secret: bytes | None = None) -> "Zkey":
+        """Phase-2 contribution (`snarkjs zkey contribute`, without its transcript): a new key with delta times s and the L
+        and H points times 1/s.  secret: 32 bytes LE in (1, r); None draws it from `secrets`.  The secret is not kept."""
+        if secret is None:
+            import secrets
+            from .circuit import FR_MODULUS
+            secret = (secrets.randbelow(FR_MODULUS - 2) + 2).to_bytes(32, "little")
+        if len(secret) != 32:
+            raise ValueError("secret must be 32 bytes")
+        err = ctypes.create_string_buffer(L.ERRCAP)
+        h = L.zke_zkey_contribute(self._h, bytes(secret), err, L.ERRCAP)
+        if not h:
+            raise L.ZkeError(err.value.decode())
+        return Zkey(self.circuit, device=self.device, _handle=h)
+
+    def contribution_report(self, prev: "Zkey", rand: bytes | None = None) -> tuple[bool, str]:
+        """(True, "") if this key follows from `prev` by phase-2 contributions, else (False, reason): the ratio check of
+        `snarkjs zkey verify`.  rand: 16 bytes that seed the random weights (default: drawn by the library)."""
+        if rand is not None and len(rand) != 16:
+            raise ValueError("rand must be 16 bytes")
+        err = ctypes.create_string_buffer(L.ERRCAP)
+        rc = L.zke_zkey_check_contribution(prev._h, self._h, bytes(rand) if rand is not None else None, err, L.ERRCAP)
+        if rc < 0:
+            raise L.ZkeError(err.value.decode())
+        return rc == 1, err.value.decode()
+
+    def check_contribution(self, prev: "Zkey", rand: bytes | None = None) -> bool:
+        return self.contribution_report(prev, rand)[0]
+
     @property
     def is_toy(self) -> bool:
         return L.zke_zkey_is_toy(self._h) == 1
@@ -98,6 +138,73 @@ class Zkey:
         if L.zke_zkey_section(self._h, sec, buf, len(buf)) < 0:
             raise L.ZkeError("section read failed")
         return buf.raw
+
+
+class _ptau_buffer:
+    """(pointer, length) of a `.ptau` given as bytes, a buffer or a path; a path is memory-mapped copy-on-write (files for
+    large domains are several GB), so nothing is read that the library does not touch."""
+
+    def __init__(self, ptau):
+        self._src, self._mm, self._arr = ptau, None, None
+
+    def __enter__(self):
+        import mmap
+        import os
+        p = self._src
+        if isinstance(p, (str, os.PathLike)):
+            with open(p, "rb") as f:
+                self._mm = mmap.mmap(f.fileno(), 0, access=mmap.ACCESS_COPY)
+            p = self._mm
+        if isinstance(p, bytes):
+            return p, len(p)
+        with memoryview(p) as mv:
+            if mv.readonly:
+                return bytes(mv), mv.nbytes
+            n = mv.nbytes
+        self._arr = (ctypes.c_char * n).from_buffer(p)
+        return ctypes.addressof(self._arr), n
+
+    def __exit__(self, *exc):
+        self._arr = None
+        if self._mm is not None:
+            self._mm.close()
+        return False
+
+
+def ptau_info(ptau, circuit: Circuit | None = None) -> dict:
+    """Structure of a prepared `.ptau` as the library reads it (host only): {"power", "sections": {type: (offset, size)}}.
+    Raises ZkeError with the library's message for a malformed file or one too small for `circuit`."""
+    power = L.c_u32()
+    offs, sizes = (L.c_u64 * 16)(), (L.c_u64 * 16)()
+    err = ctypes.create_string_buffer(L.ERRCAP)
+    with _ptau_buffer(ptau) as (ptr, n):
+        rc = L.zke_ptau_info(circuit.handle if circuit is not None else None, ptr, n, ctypes.byref(power), offs, sizes, err, L.ERRCAP)
+    if rc != 0:
+        raise L.ZkeError(err.value.decode())
+    return {"power": power.value, "sections": {s: (offs[s], sizes[s]) for s in range(16) if sizes[s] or offs[s]}}
+
+
+def ptau_toy(power: int, tau: int, alpha: int, beta: int, device: int = 0) -> bytearray:
+    """TOY prepared `.ptau` from KNOWN (tau, alpha, beta): tests and measurement only (anyone holding it can forge)."""
+    tab = b"".join(int(v).to_bytes(32, "little") for v in (tau, alpha, beta))
+    err = ctypes.create_string_buffer(L.ERRCAP)
+    n = L.zke_ptau_toy(power, tab, device, None, 0, err, L.ERRCAP)
+    if n < 0:
+        raise L.ZkeError(err.value.decode())
+    out = bytearray(n)
+    arr = (ctypes.c_char * n).from_buffer(out)
+    got = L.zke_ptau_toy(power, tab, device, ctypes.cast(arr, L.c_void_p), n, err, L.ERRCAP)
+    del arr
+    if got != n:
+        raise L.ZkeError(err.value.decode() or "ptau writer failed")
+    return out
+
+
+def verify_zkey(circuit: Circuit, ptau, zkey: Zkey, device: int | None = None, rand: bytes | None = None) -> bool:
+    """Whether `zkey` was set up for `circuit` from `ptau` (Zkey.from_ptau) followed by any number of contributions: the
+    whole delta chain collapses into one ratio, checked by Zkey.check_contribution."""
+    base = Zkey.from_ptau(circuit, ptau, device=zkey.device if device is None else device)
+    return zkey.check_contribution(base, rand)
 
 
 class Context:
