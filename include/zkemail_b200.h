@@ -161,6 +161,30 @@ int zke_zkey_check_contribution(const zke_zkey* prev, const zke_zkey* next, cons
  * zke_setup.  out == NULL: returns the size needed; -2 if cap is too small; < 0 on error. */
 int64_t zke_ptau_toy(uint32_t power, const uint8_t* tau_alpha_beta96, int device, uint8_t* out, size_t cap, char* err, size_t errcap);
 
+/* Phase 1 of the Powers-of-Tau ceremony (ptau.cu).  An UNPREPARED image holds sections 1-7, a PREPARED one also 12-15.
+ * Every writer returns the bytes written, the size needed when out == NULL, -2 if cap is too small, -1 on error.
+ * `snarkjs powersoftau new`: unprepared image of `power` (in [1, 28]) with every point the generator.  Host only. */
+int64_t zke_ptau_new(uint32_t power, uint8_t* out, size_t cap, char* err, size_t errcap);
+/* `snarkjs powersoftau contribute` with secrets (tau, alpha, beta) (3 x 32 bytes LE, each in [2, r); NULL: drawn from
+ * /dev/urandom): tauG1[i], tauG2[i] times tau^i, alphaTauG1[i] times alpha tau^i, betaTauG1[i] times beta tau^i, betaG2
+ * times beta.  Input points are validated on the device.  The output is unprepared; sections 1 and 7 are copied byte for
+ * byte and the contribution is not recorded in section 7 (no snarkjs transcript).  receipt384 (may be NULL) receives
+ * [tau]_2, [alpha]_2, [beta]_2, the public part of the contribution that zke_ptau_verify checks. */
+int64_t zke_ptau_contribute(const void* ptau, size_t len, const uint8_t* secrets96, int device, uint8_t* out, size_t cap, uint8_t* receipt384,
+                            char* err, size_t errcap);
+/* `snarkjs powersoftau prepare phase2`: an unprepared image plus sections 12-15, the Lagrange bases of the domains 1, 2, ...,
+ * 2^power computed by inverse transforms of curve points on the device.  A power whose largest transform does not fit in
+ * the device's free memory is refused before anything is allocated. */
+int64_t zke_ptau_prepare(const void* ptau, size_t len, int device, uint8_t* out, size_t cap, char* err, size_t errcap);
+/* Wall time of this thread's last zke_ptau_prepare: the three G1 families and the G2 family. */
+int zke_ptau_prepare_timing(double* g1_ms, double* g2_ms);
+/* The algebraic part of `snarkjs powersoftau verify` on an unprepared or prepared image: points valid (G2 in the order-r
+ * subgroup), generators at index 0, consecutive powers of one tau in every family, the Lagrange sections (if present) the
+ * bases of the powers and, with prev and receipt384 (both or neither), that the file is prev's after the contribution the
+ * receipt describes.  Weights derived from rand16 (NULL: /dev/urandom).  1 ok, 0 rejected with the reason in err, < 0 on error. */
+int zke_ptau_verify(const void* ptau, size_t len, const void* prev, size_t prev_len, const uint8_t* receipt384, const uint8_t* rand16,
+                    int device, char* err, size_t errcap);
+
 /* ---------------------------------------------------------------------------------------------------
  * Contexts: circuit (+ optional proving key) resident on one GPU with work buffers for `max_batch` emails.
  * One host thread per context (or external locking).  All calls are synchronous at the ABI.

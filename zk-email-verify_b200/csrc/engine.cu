@@ -1757,3 +1757,4 @@ int zke_shard_combine_raw(const uint8_t* key_points, const uint8_t* partials, in
 // Key construction from a Powers-of-Tau file, phase-2 contributions and their check: part of this translation unit,
 // because it builds zke_zkey objects the same way do_setup / do_zkey_load do.
 #include "setup.cu"
+#include "ptau.cu"

@@ -34,6 +34,7 @@ struct PtauView {
     uint32_t power = 0, ceremony_power = 0;
     SecView sec[16];
     const uint8_t* base = nullptr;
+    bool prepared = false;   // sections 12-15 present
 };
 
 const char* ptau_section_name(int s) {
@@ -60,8 +61,9 @@ const int PTAU_POINT_SECTIONS[] = {2, 3, 4, 5, 6, 12, 13, 14, 15};
 const size_t PTAU_HEADER_BYTES = 4 + 32 + 4 + 4;
 const uint32_t PTAU_MAX_POWER = 28;
 
-// Structure only (sizes, modulus, power); the points are validated on the device where they are used.
-PtauView parse_ptau(const uint8_t* b, size_t len) {
+// Structure only (sizes, modulus, power); the points are validated on the device where they are used.  With
+// lagrange_optional, sections 12-15 may be absent (an unprepared file), but only all four together.
+PtauView parse_ptau(const uint8_t* b, size_t len, bool lagrange_optional = false) {
     PtauView v;
     v.base = b;
     if (!b || len < 12 || memcmp(b, "ptau", 4) != 0) throw std::runtime_error("not a .ptau file (bad magic)");
@@ -87,7 +89,9 @@ PtauView parse_ptau(const uint8_t* b, size_t len) {
     v.power = rd32(h.p + 36);
     v.ceremony_power = rd32(h.p + 40);
     if (v.power < 1 || v.power > PTAU_MAX_POWER) throw std::runtime_error(".ptau power " + std::to_string(v.power) + " is outside [1, 28]");
+    v.prepared = v.sec[12].p || v.sec[13].p || v.sec[14].p || v.sec[15].p;
     for (int s : PTAU_POINT_SECTIONS) {
+        if (lagrange_optional && s >= 12 && !v.prepared) continue;
         if (!v.sec[s].p) throw std::runtime_error(".ptau section " + std::to_string(s) + " (" + ptau_section_name(s) + ") is missing");
         const size_t want = ptau_section_bytes(s, v.power);
         if (v.sec[s].n != want)

@@ -106,6 +106,11 @@ zke_zkey_from_ptau_timing = _sig("zke_zkey_from_ptau_timing", c_int, [ctypes.POI
 zke_zkey_contribute = _sig("zke_zkey_contribute", c_void_p, [c_void_p, c_void_p, c_char_p, c_size_t])
 zke_zkey_check_contribution = _sig("zke_zkey_check_contribution", c_int, [c_void_p, c_void_p, c_void_p, c_char_p, c_size_t])
 zke_ptau_toy = _sig("zke_ptau_toy", c_i64, [c_u32, c_void_p, c_int, c_void_p, c_size_t, c_char_p, c_size_t])
+zke_ptau_new = _sig("zke_ptau_new", c_i64, [c_u32, c_void_p, c_size_t, c_char_p, c_size_t])
+zke_ptau_contribute = _sig("zke_ptau_contribute", c_i64, [c_void_p, c_size_t, c_void_p, c_int, c_void_p, c_size_t, c_void_p, c_char_p, c_size_t])
+zke_ptau_prepare = _sig("zke_ptau_prepare", c_i64, [c_void_p, c_size_t, c_int, c_void_p, c_size_t, c_char_p, c_size_t])
+zke_ptau_prepare_timing = _sig("zke_ptau_prepare_timing", c_int, [ctypes.POINTER(ctypes.c_double), ctypes.POINTER(ctypes.c_double)])
+zke_ptau_verify = _sig("zke_ptau_verify", c_int, [c_void_p, c_size_t, c_void_p, c_size_t, c_void_p, c_void_p, c_int, c_char_p, c_size_t])
 zke_selftest_fpmul_hint =_sig("zke_selftest_fpmul_hint", c_int, [c_u32, c_u32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p])
 
 (SEC_ALPHA1, SEC_BETA1, SEC_DELTA1, SEC_BETA2, SEC_GAMMA2, SEC_DELTA2) = (101, 102, 103, 104, 105, 106)

@@ -200,6 +200,72 @@ def ptau_toy(power: int, tau: int, alpha: int, beta: int, device: int = 0) -> by
     return out
 
 
+def _ptau_write(call) -> bytearray:
+    """Runs a `.ptau` writer of the C ABI twice: for its size (out = NULL), then into a new bytearray."""
+    err = ctypes.create_string_buffer(L.ERRCAP)
+    n = call(None, 0, err)
+    if n < 0:
+        raise L.ZkeError(err.value.decode())
+    out = bytearray(n)
+    arr = (ctypes.c_char * n).from_buffer(out)
+    got = call(ctypes.cast(arr, L.c_void_p), n, err)
+    del arr
+    if got != n:
+        raise L.ZkeError(err.value.decode() or "ptau writer failed")
+    return out
+
+
+def ptau_new(power: int) -> bytearray:
+    """`snarkjs powersoftau new`: an unprepared `.ptau` (sections 1-7) of `power` whose points are all the generators."""
+    return _ptau_write(lambda out, cap, err: L.zke_ptau_new(power, out, cap, err, L.ERRCAP))
+
+
+def ptau_contribute(ptau, secrets: tuple | None = None, device: int = 0) -> tuple[bytearray, bytes]:
+    """`snarkjs powersoftau contribute` (without its transcript): (new unprepared `.ptau`, receipt).  secrets: (tau, alpha,
+    beta) ints in [2, r); None draws them from the OS.  The receipt, [tau]_2 | [alpha]_2 | [beta]_2 (384 bytes), is the
+    public part of the contribution: verify_ptau(new, prev=ptau, receipt=receipt) checks that `new` builds on `ptau`."""
+    tab = None if secrets is None else b"".join(int(v).to_bytes(32, "little") for v in secrets)
+    if tab is not None and len(tab) != 96:
+        raise ValueError("secrets must be three integers below 2^256")
+    receipt = ctypes.create_string_buffer(384)
+    with _ptau_buffer(ptau) as (ptr, n):
+        out = _ptau_write(lambda o, cap, err: L.zke_ptau_contribute(ptr, n, tab, device, o, cap, receipt if o else None, err, L.ERRCAP))
+    return out, receipt.raw
+
+
+def ptau_prepare(ptau, device: int = 0) -> bytearray:
+    """`snarkjs powersoftau prepare phase2`: the unprepared `.ptau` plus its Lagrange sections 12-15, computed on the GPU."""
+    with _ptau_buffer(ptau) as (ptr, n):
+        return _ptau_write(lambda out, cap, err: L.zke_ptau_prepare(ptr, n, device, out, cap, err, L.ERRCAP))
+
+
+def ptau_report(ptau, prev=None, receipt: bytes | None = None, device: int = 0, rand: bytes | None = None) -> tuple[bool, str]:
+    """(True, "") if `ptau` (unprepared or prepared) passes the algebraic checks of `snarkjs powersoftau verify`, else
+    (False, reason): valid points, generators at index 0, consecutive powers of one tau in every family, the Lagrange
+    sections (if present) the bases of those powers and, with `prev` and `receipt` (both or neither), that `ptau` is `prev`
+    after the contribution the receipt describes.  rand: 16 bytes that seed the random weights (default: the library's)."""
+    if (prev is None) != (receipt is None):
+        raise ValueError("prev and receipt go together")
+    if receipt is not None and len(receipt) != 384:
+        raise ValueError("receipt must be 384 bytes")
+    if rand is not None and len(rand) != 16:
+        raise ValueError("rand must be 16 bytes")
+    err = ctypes.create_string_buffer(L.ERRCAP)
+    with _ptau_buffer(ptau) as (ptr, n):
+        if prev is None:
+            rc = L.zke_ptau_verify(ptr, n, None, 0, None, bytes(rand) if rand is not None else None, device, err, L.ERRCAP)
+        else:
+            with _ptau_buffer(prev) as (pptr, pn):
+                rc = L.zke_ptau_verify(ptr, n, pptr, pn, bytes(receipt), bytes(rand) if rand is not None else None, device, err, L.ERRCAP)
+    if rc < 0:
+        raise L.ZkeError(err.value.decode())
+    return rc == 1, err.value.decode()
+
+
+def verify_ptau(ptau, prev=None, receipt: bytes | None = None, device: int = 0, rand: bytes | None = None) -> bool:
+    return ptau_report(ptau, prev, receipt, device, rand)[0]
+
+
 def verify_zkey(circuit: Circuit, ptau, zkey: Zkey, device: int | None = None, rand: bytes | None = None) -> bool:
     """Whether `zkey` was set up for `circuit` from `ptau` (Zkey.from_ptau) followed by any number of contributions: the
     whole delta chain collapses into one ratio, checked by Zkey.check_contribution."""
