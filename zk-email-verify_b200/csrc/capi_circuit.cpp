@@ -17,15 +17,18 @@ void set_err(char* err, size_t cap, const std::string& msg) {
     memcpy(err, msg.data(), n);
     err[n] = 0;
 }
-void random_scalar(U256& out) {
+void random_bytes(void* out, size_t n) {
     FILE* f = fopen("/dev/urandom", "rb");
     if (!f) throw std::runtime_error("cannot open /dev/urandom");
-    for (;;) {
-        if (fread(out.v, 1, 32, f) != 32) { fclose(f); throw std::runtime_error("short read from /dev/urandom"); }
-        out.v[3] &= 0x3FFFFFFFFFFFFFFFull;   // 254 bits, then rejection
-        if (u256_cmp(out, fr_params().p) < 0) break;
-    }
+    const bool got = fread(out, 1, n, f) == n;
     fclose(f);
+    if (!got) throw std::runtime_error("short read from /dev/urandom");
+}
+void random_scalar(U256& out) {
+    do {
+        random_bytes(out.v, 32);
+        out.v[3] &= 0x3FFFFFFFFFFFFFFFull;   // 254 bits, then rejection
+    } while (u256_cmp(out, fr_params().p) >= 0);
 }
 }  // namespace zke
 

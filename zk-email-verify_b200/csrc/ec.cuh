@@ -123,5 +123,29 @@ typedef Affine<Fq2> G2Affine;
 typedef XYZZ<Fq> G1XYZZ;
 typedef XYZZ<Fq2> G2XYZZ;
 
+// [k] P for a scalar in standard form (nbits low bits), XYZZ result
+template <class F>
+__device__ XYZZ<F> scalar_mul(const Affine<F>& p, const uint32_t* k, int nbits) {
+    XYZZ<F> acc = XYZZ<F>::inf();
+    for (int i = nbits - 1; i >= 0; --i) {
+        acc.dbl();
+        if ((k[i >> 5] >> (i & 31)) & 1) acc.madd(p, false);
+    }
+    return acc;
+}
+
+// order-r subgroup membership by [r] Q == O (as pairing_host.cpp's g2_in_subgroup); Q must be on the twist.  `inline`
+// for the linkage only: engine.cu and verify.cu both define it.
+inline __device__ __noinline__ bool g2_in_subgroup(const G2Affine& q) {
+    if (q.is_inf()) return true;
+    const FieldConsts& C = FrTag::C();
+    G2XYZZ acc = G2XYZZ::inf();
+    for (int i = 253; i >= 0; --i) {      // r < 2^254
+        acc.dbl();
+        if ((C.mod[i >> 5] >> (i & 31)) & 1) acc.madd(q, false);
+    }
+    return acc.is_inf();
+}
+
 }  // namespace dev
 }  // namespace zke

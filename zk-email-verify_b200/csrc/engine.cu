@@ -13,9 +13,11 @@ ZKE_DEFINE_CONSTANT_UPLOAD(upload_constants_engine)
 cudaError_t upload_constants_msm_g1(const FieldConsts*, const FieldConsts*);
 cudaError_t upload_constants_msm_g2(const FieldConsts*, const FieldConsts*);
 cudaError_t upload_constants_fixed_base(const FieldConsts*, const FieldConsts*);
+cudaError_t upload_constants_verify(const FieldConsts*, const FieldConsts*);
 } }
 
 #include "../../include/zkemail_b200.h"
+#include "cuda_host.hpp"
 #include "engine.hpp"
 #include "ec_host.hpp"
 #include "setup_host.hpp"
@@ -30,32 +32,23 @@ cudaError_t upload_constants_fixed_base(const FieldConsts*, const FieldConsts*);
 
 using namespace zke;
 
-#define CUDA_OK(expr) do { cudaError_t e_ = (expr); if (e_ != cudaSuccess) throw std::runtime_error(std::string("CUDA error: ") + cudaGetErrorString(e_) + " at " #expr); } while (0)
+void zke::select_device(int device) {
+    int n = 0;
+    if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0) throw std::runtime_error("no CUDA device available (this library has no CPU fallback)");
+    if (device < 0 || device >= n) throw std::runtime_error("bad device index");
+    CUDA_OK(cudaSetDevice(device));
+    dev::FieldConsts fr, fq;
+    fill_consts(fr, fr_params());
+    fill_consts(fq, fq_params());
+    CUDA_OK(dev::upload_constants_engine(&fr, &fq));
+    CUDA_OK(dev::upload_constants_msm_g1(&fr, &fq));
+    CUDA_OK(dev::upload_constants_msm_g2(&fr, &fq));
+    CUDA_OK(dev::upload_constants_fixed_base(&fr, &fq));
+    CUDA_OK(dev::upload_constants_verify(&fr, &fq));
+    CUDA_OK(dev::configure_witness_kernel());   // per-device function attribute (> 48 KB dynamic shared memory)
+}
 
 namespace {
-
-struct DevBuf {
-    uint8_t* p = nullptr;
-    size_t bytes = 0;
-    DevBuf() {}
-    DevBuf(const DevBuf&) = delete;
-    DevBuf& operator=(const DevBuf&) = delete;
-    ~DevBuf() { release(); }
-    void alloc(size_t n) { release(); if (n) { CUDA_OK(cudaMalloc(&p, n)); bytes = n; } }
-    void release() { if (p) cudaFree(p); p = nullptr; bytes = 0; }
-    template <class T> void upload(const std::vector<T>& v) {
-        alloc(v.size() * sizeof(T));
-        if (!v.empty()) CUDA_OK(cudaMemcpy(p, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice));
-    }
-};
-
-void fill_consts(dev::FieldConsts& c, const FieldParams& p) {
-    memcpy(c.mod, p.p.v, 32); memcpy(c.r, p.r.v, 32); memcpy(c.r2, p.r2.v, 32);
-    c.inv = (uint32_t)p.inv;
-    U256 zero = {{0, 0, 0, 0}}, n;
-    u256_sub(n, zero, p.p);          // 2^256 - p
-    memcpy(c.nmod, n.v, 32);
-}
 
 // Fixed-operand form of a constant w (ff.cuh: Fp::mul_shoup): {w in standard form, floor(w 2^256 / r)}.  With
 // w 2^256 = q r + rem the remainder is the Montgomery image of w, so q = (w 2^256 - rem) / r exactly, and an exact
@@ -89,24 +82,6 @@ const U256& fr_neg_inv256() {     // -r^-1 mod 2^256 (Newton iteration from the 
     return v;
 }
 ShoupPair shoup_pair(const Fr& w) { return ShoupPair{w.to_u256(), mul_lo256(w.m, fr_neg_inv256())}; }
-
-void select_device(int device) {
-    int n = 0;
-    if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0) throw std::runtime_error("no CUDA device available (this library has no CPU fallback)");
-    if (device < 0 || device >= n) throw std::runtime_error("bad device index");
-    CUDA_OK(cudaSetDevice(device));
-    dev::FieldConsts fr, fq;
-    fill_consts(fr, fr_params());
-    fill_consts(fq, fq_params());
-    CUDA_OK(dev::upload_constants_engine(&fr, &fq));
-    CUDA_OK(dev::upload_constants_msm_g1(&fr, &fq));
-    CUDA_OK(dev::upload_constants_msm_g2(&fr, &fq));
-    CUDA_OK(dev::upload_constants_fixed_base(&fr, &fq));
-    CUDA_OK(dev::configure_witness_kernel());   // per-device function attribute (> 48 KB dynamic shared memory)
-}
-
-// launch-configuration errors are not sticky: pick them up right after the launches of a stage
-#define CHECK_LAUNCH() CUDA_OK(cudaGetLastError())
 
 // 32 x 256 window table of multiples of a generator, affine Montgomery, entry d = 0 is infinity
 template <class F>
@@ -336,29 +311,58 @@ static zke_zkey* do_setup(const zke_circuit* zc, uint64_t seed, int device) {
 // snarkjs 0.5.0 (SURVEY 8(b)); the call sites are chunked-zkey.ts:80-84 and UsageGuide/README.md:139-195.
 namespace {
 struct SecView { const uint8_t* p = nullptr; size_t n = 0; };
+struct BinSection { uint32_t type; SecView view; };
 
 uint32_t rd32(const uint8_t* p) { uint32_t v; memcpy(&v, p, 4); return v; }
 uint64_t rd64(const uint8_t* p) { uint64_t v; memcpy(&v, p, 8); return v; }
 
-void split_container(const uint8_t* b, size_t len, SecView sec[11]) {
-    if (!b || len < 12 || memcmp(b, "zkey", 4) != 0) throw std::runtime_error("not a .zkey file (bad magic)");
-    if (rd32(b + 4) != 1) throw std::runtime_error("unsupported .zkey version");
+// The sections of a container of len >= 12 bytes, in file order.  The caller checks the magic and the version first,
+// and the section types and contents after; `file` (".zkey", ...) names the format in the truncation errors.
+std::vector<BinSection> binfile_sections(const uint8_t* b, size_t len, const char* file) {
+    std::vector<BinSection> out;
     const uint32_t n_sec = rd32(b + 8);
     size_t pos = 12;
     for (uint32_t i = 0; i < n_sec; ++i) {
-        if (pos + 12 > len) throw std::runtime_error("truncated .zkey (section header)");
+        if (len - pos < 12) throw std::runtime_error(std::string("truncated ") + file + " (section header)");
         const uint32_t type = rd32(b + pos);
         const uint64_t size = rd64(b + pos + 4);
         pos += 12;
-        if (size > len - pos) throw std::runtime_error("truncated .zkey (section " + std::to_string(type) + ")");
-        if (type >= 1 && type <= 10) sec[type] = SecView{b + pos, (size_t)size};
+        if (size > len - pos) throw std::runtime_error(std::string("truncated ") + file + " (section " + std::to_string(type) + ")");
+        out.push_back(BinSection{type, SecView{b + pos, (size_t)size}});
         pos += (size_t)size;
     }
+    return out;
 }
 
-template <class F> __device__ __forceinline__ bool canonical(const F& x);
-template <> __device__ __forceinline__ bool canonical<dev::Fq>(const dev::Fq& x) { dev::Fq t = x; t.reduce_once(); return t == x; }
-template <> __device__ __forceinline__ bool canonical<dev::Fq2>(const dev::Fq2& x) { return canonical(x.c0) && canonical(x.c1); }
+// appends iden3 binfile pieces to a caller buffer
+struct BinWriter {
+    uint8_t* p;
+    void u32(uint32_t v) { memcpy(p, &v, 4); p += 4; }
+    void u64(uint64_t v) { memcpy(p, &v, 8); p += 8; }
+    void bytes(const void* src, size_t n) { memcpy(p, src, n); p += n; }
+    void header(const char* magic, uint32_t version, uint32_t n_sections) { bytes(magic, 4); u32(version); u32(n_sections); }
+    void section(int s, size_t size) { u32((uint32_t)s); u64(size); }
+};
+
+void split_container(const uint8_t* b, size_t len, SecView sec[11]) {
+    if (!b || len < 12 || memcmp(b, "zkey", 4) != 0) throw std::runtime_error("not a .zkey file (bad magic)");
+    if (rd32(b + 4) != 1) throw std::runtime_error("unsupported .zkey version");
+    for (const BinSection& s : binfile_sections(b, len, ".zkey"))
+        if (s.type >= 1 && s.type <= 10) sec[s.type] = s.view;
+}
+
+// Runs launch(flag) for a kernel that atomicMin's the index of each failing item into *flag (device); returns the
+// smallest such index, or -1 if none failed.
+template <class Launch>
+int64_t first_flagged(uint32_t* flag, Launch launch) {
+    CUDA_OK(cudaMemset(flag, 0xff, 4));
+    launch(flag);
+    ZKE_COUNT_LAUNCH(1);
+    CHECK_LAUNCH();
+    uint32_t first = 0;
+    CUDA_OK(cudaMemcpy(&first, flag, 4, cudaMemcpyDeviceToHost));
+    return first == 0xffffffffu ? -1 : (int64_t)first;
+}
 
 // every point either all-zero (infinity) or on y^2 = x^3 + b with canonical (< q) coordinates
 template <class F>
@@ -367,26 +371,17 @@ __global__ void validate_points_kernel(const uint8_t* __restrict__ pts, uint32_t
     if (i >= n) return;
     const dev::Affine<F> p = dev::Affine<F>::load(pts + sizeof(dev::Affine<F>) * (size_t)i);
     if (p.is_inf()) return;
-    if (!canonical(p.x) || !canonical(p.y) || !(p.y.sqr() == p.x.sqr() * p.x + b)) atomicMin(bad, i);
+    if (!dev::below_modulus(p.x) || !dev::below_modulus(p.y) || !(p.y.sqr() == p.x.sqr() * p.x + b)) atomicMin(bad, i);
 }
 
+// -1 if every point of pts[0, n) (device) passes validate_points_kernel, else the first index that does not
 template <class F, class HostF>
-void validate_points(const uint8_t* pts, size_t n, const HostF& b_host, const char* what, uint32_t* flag_dev, const char* file = ".zkey") {
-    if (!n) return;
+int64_t first_invalid_point(const uint8_t* pts, size_t n, const HostF& b_host, uint32_t* flag) {
+    if (!n) return -1;
     F b;
     static_assert(sizeof(F) == sizeof(HostF), "host / device field images differ");
     memcpy(&b, &b_host, sizeof(F));
-    CUDA_OK(cudaMemset(flag_dev, 0xff, 4));
-    validate_points_kernel<F><<<(unsigned)((n + 127) / 128), 128>>>(pts, (uint32_t)n, b, flag_dev);
-    ZKE_COUNT_LAUNCH(1);
-    CHECK_LAUNCH();
-    uint32_t bad = 0;
-    CUDA_OK(cudaMemcpy(&bad, flag_dev, 4, cudaMemcpyDeviceToHost));
-    if (bad != 0xffffffffu) throw std::runtime_error(std::string(file) + " section " + what + ": point " + std::to_string(bad) + " is not on the curve");
-}
-template <class F, class HostF>
-void validate_points(const DevBuf& buf, size_t n, const HostF& b_host, const char* what, uint32_t* flag_dev) {
-    validate_points<F>(buf.p, n, b_host, what, flag_dev);
+    return first_flagged(flag, [&](uint32_t* f) { validate_points_kernel<F><<<(unsigned)((n + 127) / 128), 128>>>(pts, (uint32_t)n, b, f); });
 }
 
 Fq2 g2_twist_b() { return Fq2{Fq::from_u64(3), Fq::zero()} * Fq2{Fq::from_u64(9), Fq::one()}.inv(); }
@@ -483,15 +478,19 @@ static zke_zkey* do_zkey_load(const SecView sec[11], int device) {
         if (skip) CUDA_OK(cudaMemset(dst.p, 0, skip));
         if (bytes) CUDA_OK(cudaMemcpy(dst.p + skip, src, bytes, cudaMemcpyHostToDevice));
     };
-    up(zk->A, sec[5].p, sec[5].n, 0);   validate_points<dev::Fq>(zk->A, m, b1, "5 (A)", (uint32_t*)flag.p);
-    up(zk->B1, sec[6].p, sec[6].n, 0);  validate_points<dev::Fq>(zk->B1, m, b1, "6 (B1)", (uint32_t*)flag.p);
-    up(zk->B2, sec[7].p, sec[7].n, 0);  validate_points<dev::Fq2>(zk->B2, m, b2, "7 (B2)", (uint32_t*)flag.p);
+    auto refuse = [](int64_t bad, const char* what) {
+        if (bad >= 0) throw std::runtime_error(std::string(".zkey section ") + what + ": point " + std::to_string(bad) + " is not on the curve");
+    };
+    uint32_t* fl = (uint32_t*)flag.p;
+    up(zk->A, sec[5].p, sec[5].n, 0);   refuse(first_invalid_point<dev::Fq>(zk->A.p, m, b1, fl), "5 (A)");
+    up(zk->B1, sec[6].p, sec[6].n, 0);  refuse(first_invalid_point<dev::Fq>(zk->B1.p, m, b1, fl), "6 (B1)");
+    up(zk->B2, sec[7].p, sec[7].n, 0);  refuse(first_invalid_point<dev::Fq2>(zk->B2.p, m, b2, fl), "7 (B2)");
     up(zk->C, sec[8].p, sec[8].n, (size_t)(l + 1) * 64);   // C / "L": infinity for the public signals
-    validate_points<dev::Fq>(zk->C, m, b1, "8 (C)", (uint32_t*)flag.p);
+    refuse(first_invalid_point<dev::Fq>(zk->C.p, m, b1, fl), "8 (C)");
     h_table_config(zk.get(), N);
     zk->H.alloc((size_t)zk->h_levels * N * sizeof(dev::G1Affine));
     CUDA_OK(cudaMemcpy(zk->H.p, sec[9].p, N * 64, cudaMemcpyHostToDevice));
-    validate_points<dev::Fq>(zk->H, N, b1, "9 (H)", (uint32_t*)flag.p);
+    refuse(first_invalid_point<dev::Fq>(zk->H.p, N, b1, fl), "9 (H)");
     scratch.alloc((size_t)SETUP_SLAB * sizeof(dev::G1XYZZ));
     build_h_levels(zk.get(), N, scratch.p, nullptr);
     return zk.release();
@@ -517,18 +516,14 @@ static int64_t do_zkey_write(const zke_zkey* zk, const zke_circuit* zc, uint8_t*
     if (!out) return (int64_t)total;
     if (cap < total) return -2;
     CUDA_OK(cudaSetDevice(zk->device));
-    uint8_t* p = out;
-    auto w32 = [&](uint32_t v) { memcpy(p, &v, 4); p += 4; };
-    auto w64 = [&](uint64_t v) { memcpy(p, &v, 8); p += 8; };
-    auto wraw = [&](const void* src, size_t n) { memcpy(p, src, n); p += n; };
-    auto sec_hdr = [&](int s) { w32((uint32_t)s); w64(sizes[s]); };
-    memcpy(p, "zkey", 4); p += 4; w32(1); w32(10);
-    sec_hdr(1); w32(1);
-    sec_hdr(2);
-    w32(32); wraw(fq_params().p.v, 32); w32(32); wraw(fr_params().p.v, 32); w32(m); w32(l); w32((uint32_t)N);
-    wraw(&zk->alpha1, 64); wraw(&zk->beta1, 64); wraw(&zk->beta2, 128); wraw(&zk->gamma2, 128); wraw(&zk->delta1, 64); wraw(&zk->delta2, 128);
-    sec_hdr(3); wraw(zk->ic.data(), (size_t)(l + 1) * 64);
-    sec_hdr(4); w32((uint32_t)n_rec);
+    BinWriter w{out};
+    w.header("zkey", 1, 10);
+    w.section(1, sizes[1]); w.u32(1);
+    w.section(2, sizes[2]);
+    w.u32(32); w.bytes(fq_params().p.v, 32); w.u32(32); w.bytes(fr_params().p.v, 32); w.u32(m); w.u32(l); w.u32((uint32_t)N);
+    w.bytes(&zk->alpha1, 64); w.bytes(&zk->beta1, 64); w.bytes(&zk->beta2, 128); w.bytes(&zk->gamma2, 128); w.bytes(&zk->delta1, 64); w.bytes(&zk->delta2, 128);
+    w.section(3, sizes[3]); w.bytes(zk->ic.data(), (size_t)(l + 1) * 64);
+    w.section(4, sizes[4]); w.u32((uint32_t)n_rec);
     {
         const std::vector<U256>& coefs = zk->has_coefs ? zk->coefs : c->coefs;
         const Fr r_elem = Fr::from_u256(fr_params().r);
@@ -537,7 +532,7 @@ static int64_t do_zkey_write(const zke_zkey* zk, const zke_circuit* zc, uint8_t*
         for (size_t i = 0; i < coefs.size(); ++i) stored[i] = (Fr::from_u256(coefs[i]) * r2).to_u256();
         auto rows = [&](uint32_t mat, const std::vector<uint32_t>& ptr, const std::vector<uint32_t>& var, const std::vector<uint32_t>& coef, size_t n_rows) {
             for (size_t row = 0; row < n_rows; ++row)
-                for (uint32_t k = ptr[row]; k < ptr[row + 1]; ++k) { w32(mat); w32((uint32_t)row); w32(var[k]); wraw(stored[coef[k]].v, 32); }
+                for (uint32_t k = ptr[row]; k < ptr[row + 1]; ++k) { w.u32(mat); w.u32((uint32_t)row); w.u32(var[k]); w.bytes(stored[coef[k]].v, 32); }
         };
         if (zk->has_coefs) {
             rows(0, zk->a_ptr, zk->a_var, zk->a_coef, N);
@@ -546,17 +541,17 @@ static int64_t do_zkey_write(const zke_zkey* zk, const zke_circuit* zc, uint8_t*
             rows(0, c->a_ptr, c->a_var, c->a_coef, c->n_constraints);
             rows(1, c->b_ptr, c->b_var, c->b_coef, c->n_constraints);
             const U256 one_r2 = r2.to_u256();
-            for (uint32_t j = 0; j <= l; ++j) { w32(0); w32(c->n_constraints + j); w32(j); wraw(one_r2.v, 32); }
+            for (uint32_t j = 0; j <= l; ++j) { w.u32(0); w.u32(c->n_constraints + j); w.u32(j); w.bytes(one_r2.v, 32); }
         }
     }
     auto dev_sec = [&](int s, const DevBuf& b, size_t skip) {
-        sec_hdr(s);
-        if (sizes[s]) CUDA_OK(cudaMemcpy(p, b.p + skip, sizes[s], cudaMemcpyDeviceToHost));
-        p += sizes[s];
+        w.section(s, sizes[s]);
+        if (sizes[s]) CUDA_OK(cudaMemcpy(w.p, b.p + skip, sizes[s], cudaMemcpyDeviceToHost));
+        w.p += sizes[s];
     };
     dev_sec(5, zk->A, 0); dev_sec(6, zk->B1, 0); dev_sec(7, zk->B2, 0); dev_sec(8, zk->C, (size_t)(l + 1) * 64); dev_sec(9, zk->H, 0);
-    sec_hdr(10); memset(p, 0, 68); p += 68;    // circuit hash placeholder, zero contributions
-    return (int64_t)(p - out);
+    w.section(10, sizes[10]); memset(w.p, 0, 68); w.p += 68;    // circuit hash placeholder, zero contributions
+    return (int64_t)(w.p - out);
 }
 
 // ------------------------------------------------------------------------------------------------ ctx
@@ -1263,19 +1258,14 @@ static int do_prove(zke_ctx* x, zke_ctx::Slot& S, size_t batch, const uint8_t* r
 // iden3 `.wtns` v2: section 1 {u32 n8, q[n8], u32 nWitness}, section 2 nWitness x n8 bytes (standard form)
 static const uint8_t* parse_wtns(const uint8_t* b, size_t len, uint32_t expect_vars) {
     if (!b || len < 12 || memcmp(b, "wtns", 4) != 0) throw std::runtime_error("not a .wtns file (bad magic)");
-    const uint32_t n_sec = rd32(b + 8);
-    size_t pos = 12;
+    std::vector<BinSection> secs;
+    try { secs = binfile_sections(b, len, ".wtns"); }
+    catch (const std::runtime_error&) { throw std::runtime_error("truncated .wtns"); }   // without the section detail
     const uint8_t *s1 = nullptr, *s2 = nullptr;
     size_t n1 = 0, n2 = 0;
-    for (uint32_t i = 0; i < n_sec; ++i) {
-        if (pos + 12 > len) throw std::runtime_error("truncated .wtns");
-        const uint32_t type = rd32(b + pos);
-        const uint64_t size = rd64(b + pos + 4);
-        pos += 12;
-        if (size > len - pos) throw std::runtime_error("truncated .wtns");
-        if (type == 1) { s1 = b + pos; n1 = (size_t)size; }
-        if (type == 2) { s2 = b + pos; n2 = (size_t)size; }
-        pos += (size_t)size;
+    for (const BinSection& s : secs) {
+        if (s.type == 1) { s1 = s.view.p; n1 = s.view.n; }
+        if (s.type == 2) { s2 = s.view.p; n2 = s.view.n; }
     }
     if (!s1 || !s2 || n1 < 40) throw std::runtime_error(".wtns sections missing");
     if (rd32(s1) != 32 || memcmp(s1 + 4, fr_params().p.v, 32) != 0) throw std::runtime_error(".wtns is not over the BN254 scalar field");

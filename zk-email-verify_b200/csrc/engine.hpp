@@ -5,6 +5,7 @@
 
 namespace zke {
 void set_err(char* err, size_t cap, const std::string& msg);
+void random_bytes(void* out, size_t n);   // from /dev/urandom
 void random_scalar(U256& out);   // uniform in [0, r), from /dev/urandom
 }
 

@@ -710,5 +710,16 @@ struct Fq2 {
     }
 };
 
+// x < modulus (x is a canonical representative): the borrow out of x - p
+template <class Tag>
+__device__ __forceinline__ bool below_modulus(const Fp<Tag>& x) {
+    const FieldConsts& C = Tag::C();
+    (void)sub_cc(x.v[0], C.mod[0]);
+#pragma unroll
+    for (int i = 1; i < 8; ++i) (void)subc_cc(x.v[i], C.mod[i]);
+    return subc(0, 0) != 0;
+}
+__device__ __forceinline__ bool below_modulus(const Fq2& x) { return below_modulus(x.c0) && below_modulus(x.c1); }
+
 }  // namespace dev
 }  // namespace zke

@@ -314,28 +314,6 @@ __device__ __forceinline__ bool g2_on_curve(const G2Affine& a) {
     if (a.is_inf()) return true;
     return a.y.sqr() == a.x.sqr() * a.x + fq2_from(TWIST_B);
 }
-// order-r subgroup membership by [r] Q == O (as pairing_host.cpp's g2_in_subgroup); Q must be on the twist
-__device__ __noinline__ bool g2_in_subgroup(const G2Affine& q) {
-    if (q.is_inf()) return true;
-    const FieldConsts& C = FrTag::C();
-    G2XYZZ acc = G2XYZZ::inf();
-    for (int i = 253; i >= 0; --i) {      // r < 2^254
-        acc.dbl();
-        if ((C.mod[i >> 5] >> (i & 31)) & 1) acc.madd(q, false);
-    }
-    return acc.is_inf();
-}
-
-// [k] P for a scalar in standard form (nbits low bits), XYZZ result
-template <class F>
-__device__ XYZZ<F> scalar_mul(const Affine<F>& p, const uint32_t* k, int nbits) {
-    XYZZ<F> acc = XYZZ<F>::inf();
-    for (int i = nbits - 1; i >= 0; --i) {
-        acc.dbl();
-        if ((k[i >> 5] >> (i & 31)) & 1) acc.madd(p, false);
-    }
-    return acc;
-}
 __device__ __forceinline__ G1Affine g1_to_affine(const G1XYZZ& a) {
     G1Affine r;
     if (a.is_inf()) { r.x = Fq::zero(); r.y = Fq::zero(); return r; }

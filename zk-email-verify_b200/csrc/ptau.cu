@@ -21,21 +21,11 @@
 
 namespace zke { namespace dev {
 
-// first index i < n whose G2 point is not in the order-r subgroup -> atomicMin(bad).  The test is [r] Q == O, as
-// pairing.cuh's g2_in_subgroup, which belongs to verify.cu's translation unit; the points must be on the twist.
+// first index i < n whose G2 point is not in the order-r subgroup -> atomicMin(bad); the points must be on the twist
 __global__ void __launch_bounds__(128)
 g2_subgroup_kernel(const uint8_t* __restrict__ pts, uint32_t n, uint32_t* bad) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const G2Affine q = G2Affine::load(pts + sizeof(G2Affine) * (size_t)i);
-    if (q.is_inf()) return;
-    const FieldConsts& C = FrTag::C();
-    G2XYZZ acc = G2XYZZ::inf();
-    for (int b = 253; b >= 0; --b) {      // r < 2^254
-        acc.dbl();
-        if ((C.mod[b >> 5] >> (b & 31)) & 1) acc.madd(q, false);
-    }
-    if (!acc.is_inf()) atomicMin(bad, i);
+    if (i < n && !g2_in_subgroup(G2Affine::load(pts + sizeof(G2Affine) * (size_t)i))) atomicMin(bad, i);
 }
 
 } }  // namespace zke::dev
@@ -47,74 +37,22 @@ const int PTAU_PHASE1_SECTIONS[] = {2, 3, 4, 5, 6};
 size_t ptau_point_bytes(int s) { return s == 3 || s == 6 || s == 13 ? 128 : 64; }
 std::string ptau_sec_label(int s) { return "section " + std::to_string(s) + " (" + ptau_section_name(s) + ")"; }
 
-// appends iden3 binfile pieces to a caller buffer
-struct PtauWriter {
-    uint8_t* p;
-    void u32(uint32_t v) { memcpy(p, &v, 4); p += 4; }
-    void u64(uint64_t v) { memcpy(p, &v, 8); p += 8; }
-    void bytes(const void* src, size_t n) { memcpy(p, src, n); p += n; }
-    void section(int s, size_t size) { u32((uint32_t)s); u64(size); }
-};
-
-// a contribution secret in [2, r), with zke_zkey_contribute's wording
-Fr ptau_secret(const uint8_t* b32, const char* name) {
-    U256 s;
-    memcpy(s.v, b32, 32);
-    const std::string what = std::string("contribution secret ") + name;
-    if (s.is_zero()) throw std::runtime_error(what + " is zero");
-    if (u256_cmp(s, fr_params().p) >= 0) throw std::runtime_error(what + " is not below the group order r");
-    if (s.v[0] == 1 && !s.v[1] && !s.v[2] && !s.v[3]) throw std::runtime_error(what + " is one (it would change nothing)");
-    return Fr::from_u256(s);
-}
-
-// -1 if every point of pts[0, n) is infinity or on its curve with canonical coordinates, else the first bad index
-template <class F, class HostF>
-int64_t first_bad_point(const uint8_t* pts, size_t n, const HostF& b_host, uint32_t* flag) {
-    if (!n) return -1;
-    F b;
-    static_assert(sizeof(F) == sizeof(HostF), "host / device field images differ");
-    memcpy(&b, &b_host, sizeof(F));
-    CUDA_OK(cudaMemset(flag, 0xff, 4));
-    validate_points_kernel<F><<<(unsigned)((n + 127) / 128), 128>>>(pts, (uint32_t)n, b, flag);
-    ZKE_COUNT_LAUNCH(1);
-    CHECK_LAUNCH();
-    uint32_t bad = 0;
-    CUDA_OK(cudaMemcpy(&bad, flag, 4, cudaMemcpyDeviceToHost));
-    return bad == 0xffffffffu ? -1 : (int64_t)bad;
-}
-
 // -1 if every G2 point of pts[0, n) (on the twist) lies in the order-r subgroup, else the first index that does not
 int64_t first_off_subgroup(const uint8_t* pts, size_t n, uint32_t* flag) {
     if (!n) return -1;
-    CUDA_OK(cudaMemset(flag, 0xff, 4));
-    dev::g2_subgroup_kernel<<<(unsigned)((n + 127) / 128), 128>>>(pts, (uint32_t)n, flag);
-    ZKE_COUNT_LAUNCH(1);
-    CHECK_LAUNCH();
-    uint32_t bad = 0;
-    CUDA_OK(cudaMemcpy(&bad, flag, 4, cudaMemcpyDeviceToHost));
-    return bad == 0xffffffffu ? -1 : (int64_t)bad;
+    return first_flagged(flag, [&](uint32_t* f) { dev::g2_subgroup_kernel<<<(unsigned)((n + 127) / 128), 128>>>(pts, (uint32_t)n, f); });
 }
 
 // "" if the n points of section s at pts (device; index 0 = point `first` of the section) are valid, else the reason
 std::string section_points_problem(int s, const uint8_t* pts, size_t n, size_t first, uint32_t* flag) {
     const bool g2 = ptau_point_bytes(s) == 128;
-    const int64_t bad = g2 ? first_bad_point<dev::Fq2>(pts, n, g2_twist_b(), flag) : first_bad_point<dev::Fq>(pts, n, Fq::from_u64(3), flag);
+    const int64_t bad = g2 ? first_invalid_point<dev::Fq2>(pts, n, g2_twist_b(), flag) : first_invalid_point<dev::Fq>(pts, n, Fq::from_u64(3), flag);
     if (bad >= 0) return ".ptau " + ptau_sec_label(s) + ": point " + std::to_string(first + bad) + " is not on the curve";
     if (g2) {
         const int64_t off = first_off_subgroup(pts, n, flag);
         if (off >= 0) return ".ptau " + ptau_sec_label(s) + ": point " + std::to_string(first + off) + " is not in the order-r subgroup";
     }
     return "";
-}
-
-// out[i] = k_i * in[i] for n affine points on the device (k_i: standard form, device), through `x` (n XYZZ points)
-template <class F>
-void scale_each(const uint8_t* in, size_t n, const uint8_t* k, uint8_t* x, uint8_t* out, cudaStream_t st) {
-    if (!n) return;
-    dev::scale_each_kernel<F><<<(unsigned)((n + 127) / 128), 128, 0, st>>>(in, (uint32_t)n, (const uint32_t*)k, 1, 0, x);
-    ZKE_COUNT_LAUNCH(1);
-    dev::xyzz_to_affine_batch<F>(x, (uint32_t)n, out, st);
-    CHECK_LAUNCH();
 }
 
 // Section s of the contribution: point i of `in` (host) times factor * pw[i], slab by slab, into `out` (host).
@@ -136,7 +74,7 @@ void contribute_family(int s, const uint8_t* in, size_t n, const std::vector<Fr>
         CUDA_OK(cudaMemcpy(pts.p, in + off * ps, cnt * ps, cudaMemcpyHostToDevice));
         const std::string bad = section_points_problem(s, pts.p, cnt, off, flag);
         if (!bad.empty()) throw std::runtime_error(bad);
-        scale_each<F>(pts.p, cnt, k.p, x.p, pts.p, st);
+        scale_each<F>(pts.p, cnt, k.p, 1, x.p, pts.p, st);
         CUDA_OK(cudaMemcpy(out + off * ps, pts.p, cnt * ps, cudaMemcpyDeviceToHost));
     }
 }
@@ -169,22 +107,6 @@ void lagrange_family(int s, const uint8_t* first, uint32_t power, const DevBuf& 
         CHECK_LAUNCH();
         CUDA_OK(cudaMemcpy(out + (size_t)(n - 1) * ps, a.p, n * ps, cudaMemcpyDeviceToHost));
     }
-}
-
-// sum_i w_i P_i over the affine device points P_0 .. P_{n-1} (w: standard form, below r), affine host image
-template <class F, class H>
-H weighted_sum(const uint8_t* pts, const std::vector<U256>& w) {
-    H r = H::inf();
-    const uint32_t n = (uint32_t)w.size();
-    if (!n) return r;
-    const std::vector<uint32_t> ptr = {0u, n};
-    std::vector<uint2> terms(n);
-    for (uint32_t i = 0; i < n; ++i) terms[i] = make_uint2(i, i);
-    DevBuf weights, out;
-    weights.upload(w);
-    signal_sums<F>(pts, ptr, terms, weights, out, nullptr);
-    CUDA_OK(cudaMemcpy(&r, out.p, sizeof r, cudaMemcpyDeviceToHost));
-    return r;
 }
 
 // In-place inverse DFT over Fr, natural order in and out, scaled by 1/n: a_i <- n^-1 sum_j omega^(-ij) a_j
@@ -237,8 +159,8 @@ static int64_t do_ptau_new(uint32_t power, uint8_t* out, size_t cap) {
     if (cap < total) return -2;
     const G1AffineH g1 = g1_generator();
     const G2AffineH g2 = g2_generator();
-    PtauWriter w{out};
-    w.bytes("ptau", 4); w.u32(1); w.u32(7);
+    BinWriter w{out};
+    w.header("ptau", 1, 7);
     w.section(1, PTAU_HEADER_BYTES); w.u32(32); w.bytes(fq_params().p.v, 32); w.u32(power); w.u32(power);
     for (int s : PTAU_PHASE1_SECTIONS) {
         const size_t bytes = ptau_section_bytes(s, power), ps = ptau_point_bytes(s);
@@ -266,7 +188,7 @@ static int64_t do_ptau_contribute(const uint8_t* in, size_t len, const uint8_t* 
     Fr sec[3];
     const char* names[3] = {"tau", "alpha", "beta"};
     for (int i = 0; i < 3; ++i) {
-        if (secrets96) { sec[i] = ptau_secret(secrets96 + 32 * i, names[i]); continue; }
+        if (secrets96) { sec[i] = contribution_secret(secrets96 + 32 * i, names[i]); continue; }
         U256 r;
         do random_scalar(r); while (r.v[0] < 2 && !r.v[1] && !r.v[2] && !r.v[3]);
         sec[i] = Fr::from_u256(r);
@@ -279,8 +201,8 @@ static int64_t do_ptau_contribute(const uint8_t* in, size_t len, const uint8_t* 
     DevBuf flag;
     flag.alloc(4);
 
-    PtauWriter w{out};
-    w.bytes("ptau", 4); w.u32(1); w.u32(7);
+    BinWriter w{out};
+    w.header("ptau", 1, 7);
     w.section(1, v.sec[1].n); w.bytes(v.sec[1].p, v.sec[1].n);
     {
         const std::vector<Fr> pw = powers_of(tau, 2 * n - 1);
@@ -326,8 +248,8 @@ static int64_t do_ptau_prepare(const uint8_t* in, size_t len, int device, uint8_
     flag.alloc(4);
     tw.upload(to_standard(powers_of(fr_root_of_unity(v.power).inv(), N / 2)));
 
-    PtauWriter w{out};
-    w.bytes("ptau", 4); w.u32(1); w.u32(11);
+    BinWriter w{out};
+    w.header("ptau", 1, 11);
     for (int s : {1, 2, 3, 4, 5, 6, 7}) { w.section(s, v.sec[s].n); w.bytes(v.sec[s].p, v.sec[s].n); }
     const auto t0 = std::chrono::steady_clock::now();
     double g2_ms = 0;
@@ -500,7 +422,7 @@ int zke_ptau_verify(const void* ptau, size_t len, const void* prev, size_t prev_
         if (!prev != !receipt384) throw std::runtime_error("the previous file and the receipt go together: give both or neither");
         uint8_t seed[16];
         if (rand16) memcpy(seed, rand16, 16);
-        else for (int i = 0; i < 2; ++i) { U256 r; random_scalar(r); memcpy(seed + 8 * i, &r.v[0], 8); }
+        else random_bytes(seed, 16);
         std::string why;
         const int ok = do_ptau_verify((const uint8_t*)ptau, len, (const uint8_t*)prev, prev_len, receipt384, seed, device, why);
         set_err(err, errcap, why);

@@ -11,6 +11,7 @@
 // of at most SETUP_FANIN partials each - so the constant wire, with hundreds of thousands of terms, does not serialise
 // a warp.  The key has gamma = delta = 1: anyone who knows it can forge proofs, so it reports itself as a toy until a
 // contribution replaces delta.
+#include "ec_ntt.cuh"
 #include <chrono>
 
 namespace {
@@ -68,19 +69,10 @@ PtauView parse_ptau(const uint8_t* b, size_t len, bool lagrange_optional = false
     v.base = b;
     if (!b || len < 12 || memcmp(b, "ptau", 4) != 0) throw std::runtime_error("not a .ptau file (bad magic)");
     if (rd32(b + 4) != 1) throw std::runtime_error("unsupported .ptau version " + std::to_string(rd32(b + 4)));
-    const uint32_t n_sec = rd32(b + 8);
-    size_t pos = 12;
-    for (uint32_t i = 0; i < n_sec; ++i) {
-        if (len - pos < 12) throw std::runtime_error("truncated .ptau (section header)");
-        const uint32_t type = rd32(b + pos);
-        const uint64_t size = rd64(b + pos + 4);
-        pos += 12;
-        if (size > len - pos) throw std::runtime_error("truncated .ptau (section " + std::to_string(type) + ")");
-        if (type < 16) {
-            if (v.sec[type].p) throw std::runtime_error(".ptau section " + std::to_string(type) + " appears twice");
-            v.sec[type] = SecView{b + pos, (size_t)size};
-        }
-        pos += (size_t)size;
+    for (const BinSection& s : binfile_sections(b, len, ".ptau")) {
+        if (s.type >= 16) continue;
+        if (v.sec[s.type].p) throw std::runtime_error(".ptau section " + std::to_string(s.type) + " appears twice");
+        v.sec[s.type] = s.view;
     }
     const SecView& h = v.sec[1];
     if (!h.p) throw std::runtime_error(".ptau header section 1 is missing");
@@ -172,7 +164,8 @@ static const uint32_t SETUP_CHUNK = 32;   // terms summed by one thread in the f
 static const uint32_t SETUP_FANIN = 32;   // partial sums added by one thread in each further pass
 
 // acc += coef * P for a term {point index, coefficient index}; a coefficient of magnitude 1 is one mixed addition,
-// any other a double-and-add over its bits.
+// any other a double-and-add over its bits.  The loop starts from P at the top bit rather than calling ec.cuh's
+// scalar_mul: the scalar_mul form made the device part of `from_ptau` 3.6% slower (H100 80GB HBM3, 700 W).
 template <class F>
 __device__ __forceinline__ void add_term(XYZZ<F>& acc, const uint8_t* __restrict__ points, uint2 t, const uint32_t* __restrict__ coefs) {
     const Affine<F> p = Affine<F>::load(points + sizeof(Affine<F>) * (size_t)t.x);
@@ -217,30 +210,6 @@ setup_partial_sum_kernel(const uint8_t* __restrict__ in_xyzz, const uint32_t* __
     XYZZ<F> acc = XYZZ<F>::inf();
     for (uint32_t k = ptr[s]; k < ptr[s + 1]; ++k) acc.add(XYZZ<F>::load(in_xyzz + sizeof(XYZZ<F>) * (size_t)k));
     acc.store(out_xyzz + sizeof(XYZZ<F>) * (size_t)s);
-}
-
-// One scalar shared by all points, as signed 4-bit digits (most significant first, each in [-8, 8]).
-struct SharedScalar { int8_t d[68]; int n; };
-
-// out[i] = k * in[i]: every thread runs the same digit sequence over a table of 1..8 times its own point.
-__global__ void __launch_bounds__(128)
-scale_points_kernel(const uint8_t* __restrict__ in_affine, uint32_t n, SharedScalar k, uint8_t* __restrict__ out_xyzz) {
-    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const G1Affine p = G1Affine::load(in_affine + sizeof(G1Affine) * (size_t)i);
-    G1XYZZ acc = G1XYZZ::inf();
-    if (!p.is_inf()) {
-        G1XYZZ t[8];
-        t[0] = G1XYZZ::from_affine(p);
-        t[1] = t[0]; t[1].dbl();
-        for (int j = 2; j < 8; ++j) { t[j] = t[j - 1]; t[j].madd(p, false); }
-        for (int w = 0; w < k.n; ++w) {
-            acc.dbl(); acc.dbl(); acc.dbl(); acc.dbl();
-            const int d = k.d[w];
-            if (d) { G1XYZZ q = t[(d < 0 ? -d : d) - 1]; if (d < 0) q.negate(); acc.add(q); }
-        }
-    }
-    acc.store(out_xyzz + sizeof(G1XYZZ) * (size_t)i);
 }
 
 // first index i < n with a[i] != b[i] (16-byte words) -> atomicMin(first)
@@ -303,34 +272,43 @@ void signal_sums(const uint8_t* points_dev, const std::vector<uint32_t>& sig_ptr
     CUDA_OK(cudaStreamSynchronize(st));
 }
 
-// out = k * in for n G1 points (affine, device), in slabs
-void scale_points(const uint8_t* in, size_t n, const U256& k, uint8_t* out, cudaStream_t st) {
-    dev::SharedScalar sk;
-    memset(&sk, 0, sizeof sk);
-    {   // signed 4-bit recoding, least significant first, then reversed
-        int8_t d[68];
-        int nd = 0;
-        U256 x = k;
-        while (!x.is_zero()) {   // x <- (x - d) / 16 with d = x mod 16 taken in [-8, 8)
-            int v = (int)(x.v[0] & 15);
-            if (v >= 8) { v -= 16; const U256 a = {{(uint64_t)(-v), 0, 0, 0}}; u256_add(x, x, a); }
-            else x.v[0] &= ~15ull;
-            d[nd++] = (int8_t)v;
-            for (int i = 0; i < 4; ++i) x.v[i] = (x.v[i] >> 4) | (i < 3 ? x.v[i + 1] << 60 : 0);
-        }
-        sk.n = nd;
-        for (int i = 0; i < nd; ++i) sk.d[i] = d[nd - 1 - i];
-    }
-    DevBuf scratch;
-    scratch.alloc((size_t)std::min<size_t>(SETUP_SLAB, std::max<size_t>(1, n)) * sizeof(dev::G1XYZZ));
-    for (size_t off = 0; off < n; off += SETUP_SLAB) {
-        const uint32_t cnt = (uint32_t)std::min<size_t>(SETUP_SLAB, n - off);
-        dev::scale_points_kernel<<<(cnt + 127) / 128, 128, 0, st>>>(in + 64 * off, cnt, sk, scratch.p);
-        ZKE_COUNT_LAUNCH(1);
-        dev::xyzz_to_affine_batch<dev::Fq>(scratch.p, cnt, out + 64 * off, st);
-        CHECK_LAUNCH();
-    }
-    CUDA_OK(cudaStreamSynchronize(st));
+// out[i] = k_i * in[i] for n affine points on the device (k_i = k[i * stride], standard form, device; stride 0: one
+// scalar for all), through `x` (n XYZZ points)
+template <class F>
+void scale_each(const uint8_t* in, size_t n, const uint8_t* k, uint32_t stride, uint8_t* x, uint8_t* out, cudaStream_t st) {
+    if (!n) return;
+    dev::scale_each_kernel<F><<<(unsigned)((n + 127) / 128), 128, 0, st>>>(in, (uint32_t)n, (const uint32_t*)k, stride, 0, x);
+    ZKE_COUNT_LAUNCH(1);
+    dev::xyzz_to_affine_batch<F>(x, (uint32_t)n, out, st);
+    CHECK_LAUNCH();
+}
+
+// sum_i w_i P_i over the affine device points P_0 .. P_{n-1} (w: standard form, below r), affine host image: one
+// segment of n terms {point i, weight i} through the signal sums
+template <class F, class H>
+H weighted_sum(const uint8_t* pts, const std::vector<U256>& w) {
+    H r = H::inf();
+    const uint32_t n = (uint32_t)w.size();
+    if (!n) return r;
+    const std::vector<uint32_t> ptr = {0u, n};
+    std::vector<uint2> terms(n);
+    for (uint32_t i = 0; i < n; ++i) terms[i] = make_uint2(i, i);
+    DevBuf weights, out;
+    weights.upload(w);
+    signal_sums<F>(pts, ptr, terms, weights, out, nullptr);
+    CUDA_OK(cudaMemcpy(&r, out.p, sizeof r, cudaMemcpyDeviceToHost));
+    return r;
+}
+
+// a contribution secret in [2, r); `name` (may be null) follows "contribution secret" in the messages
+Fr contribution_secret(const uint8_t* b32, const char* name = nullptr) {
+    U256 s;
+    memcpy(s.v, b32, 32);
+    const std::string what = name ? std::string("contribution secret ") + name : std::string("contribution secret");
+    if (s.is_zero()) throw std::runtime_error(what + " is zero");
+    if (u256_cmp(s, fr_params().p) >= 0) throw std::runtime_error(what + " is not below the group order r");
+    if (s.v[0] == 1 && !s.v[1] && !s.v[2] && !s.v[3]) throw std::runtime_error(what + " is one (it would change nothing)");
+    return Fr::from_u256(s);
 }
 
 bool g1_valid(const G1AffineH& p) { return u256_cmp(p.x.m, fq_params().p) < 0 && u256_cmp(p.y.m, fq_params().p) < 0 && g1_on_curve(p); }
@@ -406,12 +384,16 @@ static zke_zkey* do_zkey_from_ptau(const zke_circuit* zc, const uint8_t* file, s
     CUDA_OK(cudaMemcpy(g1b.p, ptau_basis(v, 12, log_n), N * 64, cudaMemcpyHostToDevice));
     CUDA_OK(cudaMemcpy(g1b.p + N * 64, ptau_basis(v, 14, log_n), N * 64, cudaMemcpyHostToDevice));
     CUDA_OK(cudaMemcpy(g1b.p + 2 * N * 64, ptau_basis(v, 15, log_n), N * 64, cudaMemcpyHostToDevice));
-    validate_points<dev::Fq>(g1b.p, N, b1, "12 (lTauG1)", (uint32_t*)flag.p, ".ptau");
-    validate_points<dev::Fq>(g1b.p + N * 64, N, b1, "14 (lAlphaTauG1)", (uint32_t*)flag.p, ".ptau");
-    validate_points<dev::Fq>(g1b.p + 2 * N * 64, N, b1, "15 (lBetaTauG1)", (uint32_t*)flag.p, ".ptau");
+    auto refuse = [](int64_t bad, const char* what) {
+        if (bad >= 0) throw std::runtime_error(std::string(".ptau section ") + what + ": point " + std::to_string(bad) + " is not on the curve");
+    };
+    uint32_t* fl = (uint32_t*)flag.p;
+    refuse(first_invalid_point<dev::Fq>(g1b.p, N, b1, fl), "12 (lTauG1)");
+    refuse(first_invalid_point<dev::Fq>(g1b.p + N * 64, N, b1, fl), "14 (lAlphaTauG1)");
+    refuse(first_invalid_point<dev::Fq>(g1b.p + 2 * N * 64, N, b1, fl), "15 (lBetaTauG1)");
     g2b.alloc(N * 128);
     CUDA_OK(cudaMemcpy(g2b.p, ptau_basis(v, 13, log_n), N * 128, cudaMemcpyHostToDevice));
-    validate_points<dev::Fq2>(g2b.p, N, b2, "13 (lTauG2)", (uint32_t*)flag.p, ".ptau");
+    refuse(first_invalid_point<dev::Fq2>(g2b.p, N, b2, fl), "13 (lTauG2)");
 
     signal_sums<dev::Fq>(g1b.p, a_ptr, a_terms, coefs_dev, zk->A, st);
     signal_sums<dev::Fq>(g1b.p, ab_ptr, b_terms, coefs_dev, zk->B1, st);
@@ -428,7 +410,7 @@ static zke_zkey* do_zkey_from_ptau(const zke_circuit* zc, const uint8_t* file, s
     h_table_config(zk.get(), N);
     zk->H.alloc((size_t)zk->h_levels * N * sizeof(dev::G1Affine));
     CUDA_OK(cudaMemcpy2D(zk->H.p, 64, ptau_basis(v, 12, log_n + 1) + 64, 128, 64, N, cudaMemcpyHostToDevice));
-    validate_points<dev::Fq>(zk->H.p, N, b1, "12 (lTauG1, size-2N basis)", (uint32_t*)flag.p, ".ptau");
+    refuse(first_invalid_point<dev::Fq>(zk->H.p, N, b1, fl), "12 (lTauG1, size-2N basis)");
     DevBuf scratch;
     scratch.alloc((size_t)SETUP_SLAB * sizeof(dev::G1XYZZ));
     build_h_levels(zk.get(), N, scratch.p, st);
@@ -438,11 +420,8 @@ static zke_zkey* do_zkey_from_ptau(const zke_circuit* zc, const uint8_t* file, s
 
 // ------------------------------------------------------------------------------------------------ zke_zkey_contribute
 static zke_zkey* do_zkey_contribute(const zke_zkey* prev, const uint8_t* secret32) {
-    U256 s;
-    memcpy(s.v, secret32, 32);
-    if (s.is_zero()) throw std::runtime_error("contribution secret is zero");
-    if (u256_cmp(s, fr_params().p) >= 0) throw std::runtime_error("contribution secret is not below the group order r");
-    if (s.v[0] == 1 && !s.v[1] && !s.v[2] && !s.v[3]) throw std::runtime_error("contribution secret is one (it would change nothing)");
+    const Fr sf = contribution_secret(secret32);
+    const U256 s = sf.to_u256();
     CUDA_OK(cudaSetDevice(prev->device));
     select_device(prev->device);
     const uint32_t m = prev->n_vars;
@@ -455,23 +434,27 @@ static zke_zkey* do_zkey_contribute(const zke_zkey* prev, const uint8_t* secret3
     zk->has_coefs = prev->has_coefs;
     zk->a_ptr = prev->a_ptr; zk->a_var = prev->a_var; zk->a_coef = prev->a_coef;
     zk->b_ptr = prev->b_ptr; zk->b_var = prev->b_var; zk->b_coef = prev->b_coef; zk->coefs = prev->coefs;
-    const Fr sf = Fr::from_u256(s);
     zk->delta1 = G1JacH::from_affine(prev->delta1).mul(s).to_affine();
     zk->delta2 = G2JacH::from_affine(prev->delta2).mul(s).to_affine();
-    const U256 s_inv = sf.inv().to_u256();
 
     auto copy = [&](DevBuf& dst, const DevBuf& src, size_t bytes) { dst.alloc(bytes); CUDA_OK(cudaMemcpy(dst.p, src.p, bytes, cudaMemcpyDeviceToDevice)); };
     copy(zk->A, prev->A, (size_t)m * 64);
     copy(zk->B1, prev->B1, (size_t)m * 64);
     copy(zk->B2, prev->B2, (size_t)m * 128);
     cudaStream_t st = nullptr;
+    DevBuf s_inv, scratch;
+    s_inv.upload(std::vector<U256>{sf.inv().to_u256()});
+    scratch.alloc((size_t)SETUP_SLAB * sizeof(dev::G1XYZZ));
+    auto scale = [&](const uint8_t* in, size_t n, uint8_t* out) {   // out = s^-1 in, slab by slab
+        for (size_t off = 0; off < n; off += SETUP_SLAB)
+            scale_each<dev::Fq>(in + 64 * off, std::min<size_t>(SETUP_SLAB, n - off), s_inv.p, 0, scratch.p, out + 64 * off, st);
+        CUDA_OK(cudaStreamSynchronize(st));
+    };
     zk->C.alloc((size_t)m * 64);
-    scale_points(prev->C.p, m, s_inv, zk->C.p, st);        // the public rows are infinity and stay so
+    scale(prev->C.p, m, zk->C.p);        // the public rows are infinity and stay so
     zk->cfg_h = prev->cfg_h; zk->h_levels = prev->h_levels;
     zk->H.alloc((size_t)zk->h_levels * N * sizeof(dev::G1Affine));
-    scale_points(prev->H.p, N, s_inv, zk->H.p, st);
-    DevBuf scratch;
-    scratch.alloc((size_t)SETUP_SLAB * sizeof(dev::G1XYZZ));
+    scale(prev->H.p, N, zk->H.p);
     build_h_levels(zk.get(), N, scratch.p, st);
     return zk.release();
 }
@@ -492,22 +475,6 @@ static void derive_weights(const uint8_t* rand16, size_t n, std::vector<U256>& o
         const uint64_t b = mix(k1 + 0x9E3779B97F4A7C15ull * (2 * i + 2)) ^ mix(k0 ^ (0xD1B54A32D192ED03ull * (i + 7)));
         out[i] = U256{{a, b | 1, 0, 0}};    // never zero
     }
-}
-
-// sum_i w_i P_i over n affine device points: one segment of n terms {point i, weight i} through the signal-sum kernels
-// of the key construction (double-and-add over each 128-bit weight, chunked partial sums)
-static G1JacH device_weighted_sum(const uint8_t* points, const std::vector<U256>& w, cudaStream_t st) {
-    const uint32_t n = (uint32_t)w.size();
-    if (!n) return G1JacH::inf();
-    const std::vector<uint32_t> ptr = {0u, n};
-    std::vector<uint2> terms(n);
-    for (uint32_t i = 0; i < n; ++i) terms[i] = make_uint2(i, i);
-    DevBuf weights, out;
-    weights.upload(w);
-    signal_sums<dev::Fq>(points, ptr, terms, weights, out, st);
-    G1AffineH r;
-    CUDA_OK(cudaMemcpy(&r, out.p, sizeof r, cudaMemcpyDeviceToHost));
-    return G1JacH::from_affine(r);
 }
 
 // 1: next follows from prev by one or more contributions; 0: it does not (reason in `why`)
@@ -537,13 +504,11 @@ static int do_check_contribution(const zke_zkey* a, const zke_zkey* b, const uin
     flag.alloc(4);
     auto differ = [&](const DevBuf& x, const DevBuf& y, size_t bytes, size_t point_bytes) -> int64_t {
         const uint32_t words = (uint32_t)(bytes / 16);
-        CUDA_OK(cudaMemset(flag.p, 0xff, 4));
-        if (words) dev::words_differ_kernel<<<(words + 255) / 256, 256>>>((const uint4*)x.p, (const uint4*)y.p, words, (uint32_t*)flag.p);
-        ZKE_COUNT_LAUNCH(1);
-        if (cudaError_t e = cudaGetLastError()) throw std::runtime_error(std::string("point comparison: ") + cudaGetErrorString(e));
-        uint32_t first = 0;
-        CUDA_OK(cudaMemcpy(&first, flag.p, 4, cudaMemcpyDeviceToHost));
-        return first == 0xffffffffu ? -1 : (int64_t)first * 16 / (int64_t)point_bytes;
+        if (!words) return -1;
+        const int64_t first = first_flagged((uint32_t*)flag.p, [&](uint32_t* f) {
+            dev::words_differ_kernel<<<(words + 255) / 256, 256>>>((const uint4*)x.p, (const uint4*)y.p, words, f);
+        });
+        return first < 0 ? -1 : first * 16 / (int64_t)point_bytes;
     };
     int64_t d;
     if ((d = differ(a->A, b->A, (size_t)m * 64, 64)) >= 0) { why = "A point " + std::to_string(d) + " differs"; return 0; }
@@ -564,9 +529,10 @@ static int do_check_contribution(const zke_zkey* a, const zke_zkey* b, const uin
     wh.assign(wc.begin() + m, wc.end());
     wc.resize(m);
     for (uint32_t j = 0; j <= l; ++j) wc[j] = U256{{0, 0, 0, 0}};    // the public rows of C are infinity
-    cudaStream_t st = nullptr;
-    const G1AffineH xa = device_weighted_sum(a->C.p, wc, st).add(device_weighted_sum(a->H.p, wh, st)).to_affine();
-    const G1AffineH xb = device_weighted_sum(b->C.p, wc, st).add(device_weighted_sum(b->H.p, wh, st)).to_affine();
+    auto x_of = [&](const zke_zkey* k) {
+        return G1JacH::from_affine(weighted_sum<dev::Fq, G1AffineH>(k->C.p, wc)).add(G1JacH::from_affine(weighted_sum<dev::Fq, G1AffineH>(k->H.p, wh))).to_affine();
+    };
+    const G1AffineH xa = x_of(a), xb = x_of(b);
     G1AffineH neg_xa = xa;
     neg_xa.y = neg_xa.y.neg();
     if (xa.is_inf() != xb.is_inf() || !pairing_product_is_one({{xb, b->delta2}, {neg_xa, a->delta2}})) {
@@ -618,11 +584,9 @@ static int64_t do_ptau_toy(uint32_t power, const uint8_t* tab96, int device, uin
     pts.alloc((size_t)SETUP_SLAB * sizeof(dev::G2Affine));
     cudaStream_t st = nullptr;
 
-    uint8_t* p = out;
-    auto w32 = [&](uint32_t v) { memcpy(p, &v, 4); p += 4; };
-    auto w64 = [&](uint64_t v) { memcpy(p, &v, 8); p += 8; };
-    auto sec_hdr = [&](int s) { w32((uint32_t)s); w64(sec_bytes(s)); };
-    // [k_i]_1 or [k_i]_2 for the scalars k, appended at p
+    BinWriter w{out};
+    auto sec_hdr = [&](int s) { w.section(s, sec_bytes(s)); };
+    // [k_i]_1 or [k_i]_2 for the scalars k, appended at w.p
     auto emit = [&](const std::vector<Fr>& k, bool g2) {
         const std::vector<U256> std_k = to_standard(k);
         scal.upload(std_k);
@@ -632,14 +596,14 @@ static int64_t do_ptau_toy(uint32_t power, const uint8_t* tab96, int device, uin
             if (g2) dev::fixed_base_batch<dev::Fq2>(t2.p, scal.p + 32 * off, cnt, scratch.p, pts.p, st);
             else dev::fixed_base_batch<dev::Fq>(t1.p, scal.p + 32 * off, cnt, scratch.p, pts.p, st);
             CHECK_LAUNCH();
-            CUDA_OK(cudaMemcpy(p, pts.p, cnt * ps, cudaMemcpyDeviceToHost));
-            p += cnt * ps;
+            CUDA_OK(cudaMemcpy(w.p, pts.p, cnt * ps, cudaMemcpyDeviceToHost));
+            w.p += cnt * ps;
         }
     };
     auto scaled = [](std::vector<Fr> v, const Fr& k) { for (auto& x : v) x = x * k; return v; };
 
-    memcpy(p, "ptau", 4); p += 4; w32(1); w32((uint32_t)(sizeof order / sizeof order[0]));
-    sec_hdr(1); w32(32); memcpy(p, fq_params().p.v, 32); p += 32; w32(power); w32(power);
+    w.header("ptau", 1, (uint32_t)(sizeof order / sizeof order[0]));
+    sec_hdr(1); w.u32(32); w.bytes(fq_params().p.v, 32); w.u32(power); w.u32(power);
     {
         std::vector<Fr> pw = powers_of(tau, 2 * n - 1);
         sec_hdr(2); emit(pw, false);
@@ -648,7 +612,7 @@ static int64_t do_ptau_toy(uint32_t power, const uint8_t* tab96, int device, uin
         sec_hdr(4); emit(scaled(pw, alpha), false);
         sec_hdr(5); emit(scaled(pw, beta), false);
         sec_hdr(6); emit({beta}, true);
-        sec_hdr(7); w32(0);
+        sec_hdr(7); w.u32(0);
     }
     {
         // Lagrange bases of the domains 2^0 .. 2^power at tau, back to back
@@ -666,7 +630,7 @@ static int64_t do_ptau_toy(uint32_t power, const uint8_t* tab96, int device, uin
         sec_hdr(15); emit(scaled(lag, beta), false);
     }
     CUDA_OK(cudaStreamSynchronize(st));
-    return (int64_t)(p - out);
+    return (int64_t)(w.p - out);
 }
 
 extern "C" {
@@ -710,7 +674,7 @@ int zke_zkey_check_contribution(const zke_zkey* prev, const zke_zkey* next, cons
         if (!prev || !next) throw std::runtime_error("null key");
         uint8_t seed[16];
         if (rand16) memcpy(seed, rand16, 16);
-        else for (int i = 0; i < 2; ++i) { U256 r; random_scalar(r); memcpy(seed + 8 * i, &r.v[0], 8); }
+        else random_bytes(seed, 16);
         std::string why;
         const int ok = do_check_contribution(prev, next, seed, why);
         set_err(err, errcap, why);

@@ -12,10 +12,10 @@
 // The verdicts are those of the host path (zke_verify_batch_json: groth16_verify_batch, then groth16_verify per proof).
 #include "pairing.cuh"
 #include "device_engine.cuh"
+#include "cuda_host.hpp"
 #include "../../include/zkemail_b200.h"
 #include "engine.hpp"
 #include "ec_host.hpp"
-#include <cstdio>
 #include <cstring>
 #include <memory>
 #include <stdexcept>
@@ -32,14 +32,6 @@ static const uint32_t FOLD = 32;     // elements combined per thread and level o
 
 struct FixedLines { const uint8_t* p[3]; };   // line tables of beta2, gamma2, delta2 (null: the point is at infinity)
 
-template <class Tag>
-__device__ __forceinline__ bool below_modulus(const Fp<Tag>& x) {
-    const FieldConsts& C = Tag::C();
-    (void)sub_cc(x.v[0], C.mod[0]);
-#pragma unroll
-    for (int i = 1; i < 8; ++i) (void)subc_cc(x.v[i], C.mod[i]);
-    return subc(0, 0) != 0;    // borrow: x < modulus
-}
 __device__ __forceinline__ G1Affine g1_zero() { G1Affine r; r.x = Fq::zero(); r.y = Fq::zero(); return r; }
 __device__ __forceinline__ G2Affine g2_zero() { G2Affine r; r.x = Fq2::zero(); r.y = Fq2::zero(); return r; }
 
@@ -234,48 +226,9 @@ pairing_selftest_kernel(const uint8_t* __restrict__ g1, const uint8_t* __restric
 
 using namespace zke;
 
-#define VCUDA(expr) do { cudaError_t e_ = (expr); if (e_ != cudaSuccess) throw std::runtime_error(std::string("CUDA error: ") + cudaGetErrorString(e_) + " at " #expr); } while (0)
-
 namespace {
 
-// grow-only device allocation
-struct DevMem {
-    uint8_t* p = nullptr;
-    size_t bytes = 0;
-    DevMem() {}
-    DevMem(const DevMem&) = delete;
-    DevMem& operator=(const DevMem&) = delete;
-    ~DevMem() { if (p) cudaFree(p); }
-    uint8_t* get(size_t n) {
-        if (n > bytes) {
-            if (p) cudaFree(p);
-            p = nullptr; bytes = 0;
-            VCUDA(cudaMalloc(&p, n));
-            bytes = n;
-        }
-        return p;
-    }
-};
-
-void fill_field_consts(dev::FieldConsts& c, const FieldParams& prm) {
-    memcpy(c.mod, prm.p.v, 32); memcpy(c.r, prm.r.v, 32); memcpy(c.r2, prm.r2.v, 32);
-    c.inv = (uint32_t)prm.inv;
-    U256 zero = {{0, 0, 0, 0}}, neg;
-    u256_sub(neg, zero, prm.p);
-    memcpy(c.nmod, neg.v, 32);
-}
-void use_device(int device) {
-    int count = 0;
-    if (cudaGetDeviceCount(&count) != cudaSuccess || count == 0) throw std::runtime_error("no CUDA device available (this library has no CPU fallback)");
-    if (device < 0 || device >= count) throw std::runtime_error("bad device index");
-    VCUDA(cudaSetDevice(device));
-    dev::FieldConsts fr, fq;
-    fill_field_consts(fr, fr_params());
-    fill_field_consts(fq, fq_params());
-    VCUDA(dev::upload_constants_verify(&fr, &fq));
-}
 unsigned blocks(size_t threads) { return (unsigned)((threads + dev::VERIFY_THREADS - 1) / dev::VERIFY_THREADS); }
-#define VCHECK_LAUNCH(k) do { VCUDA(cudaGetLastError()); ZKE_COUNT_LAUNCH(k); } while (0)
 
 void put_fq(std::vector<uint8_t>& out, const Fq& x) { const uint8_t* b = reinterpret_cast<const uint8_t*>(x.m.v); out.insert(out.end(), b, b + 32); }
 void put_g1(std::vector<uint8_t>& out, const G1AffineH& p) { put_fq(out, p.x); put_fq(out, p.y); }
@@ -289,7 +242,7 @@ const uint8_t* fold_all(const uint8_t* in, uint32_t count, uint32_t width, uint8
     while (count > 1) {
         const uint32_t groups = (count + dev::FOLD - 1) / dev::FOLD;
         dev::verify_fold_kernel<Op><<<blocks((size_t)groups * width), dev::VERIFY_THREADS, 0, st>>>(in, count, width, bufs[b]);
-        VCHECK_LAUNCH(1);
+        ZKE_COUNT_LAUNCH(1); CHECK_LAUNCH();
         in = bufs[b];
         b ^= 1;
         count = groups;
@@ -305,10 +258,10 @@ struct zke_verifier {
     int device = 0;
     uint32_t n_public = 0;
     cudaStream_t stream = nullptr;
-    DevMem ic, alpha, g2, lines, e_ab;
+    DevBuf ic, alpha, g2, lines, e_ab;
     dev::FixedLines fl{{nullptr, nullptr, nullptr}};
     // per-call buffers
-    DevMem proofs, publics, rand32, mont, valid, ok, neg_ra, rc, rc_s0, rc_s1, terms, terms_s0, terms_s1, products, fixed_p, f,
+    DevBuf proofs, publics, rand32, mont, valid, ok, neg_ra, rc, rc_s0, rc_s1, terms, terms_s0, terms_s1, products, fixed_p, f,
         f_s0, f_s1, flag;
     ~zke_verifier() {
         if (stream) cudaStreamDestroy(stream);
@@ -333,23 +286,23 @@ zke_verifier* zke_verifier_open(const char* vkey_json, int device, char* err, si
         std::unique_ptr<zke_verifier> v(new zke_verifier());
         v->device = device;
         v->n_public = (uint32_t)(vk.ic.size() - 1);
-        use_device(device);
-        VCUDA(cudaStreamCreateWithFlags(&v->stream, cudaStreamNonBlocking));
+        select_device(device);
+        CUDA_OK(cudaStreamCreateWithFlags(&v->stream, cudaStreamNonBlocking));
         std::vector<uint8_t> ic, alpha, g2;
         for (auto& p : vk.ic) put_g1(ic, p);
         put_g1(alpha, vk.alpha1);
         for (int k = 0; k < 3; ++k) put_g2(g2, *g2s[k]);
-        VCUDA(cudaMemcpy(v->ic.get(ic.size()), ic.data(), ic.size(), cudaMemcpyHostToDevice));
-        VCUDA(cudaMemcpy(v->alpha.get(64), alpha.data(), 64, cudaMemcpyHostToDevice));
-        VCUDA(cudaMemcpy(v->g2.get(384), g2.data(), 384, cudaMemcpyHostToDevice));
+        CUDA_OK(cudaMemcpy(v->ic.reserve(ic.size()), ic.data(), ic.size(), cudaMemcpyHostToDevice));
+        CUDA_OK(cudaMemcpy(v->alpha.reserve(64), alpha.data(), 64, cudaMemcpyHostToDevice));
+        CUDA_OK(cudaMemcpy(v->g2.reserve(384), g2.data(), 384, cudaMemcpyHostToDevice));
         const size_t table = (size_t)dev::ATE_LINES * dev::LINE_BYTES;
-        uint8_t* lines = v->lines.get(3 * table);
+        uint8_t* lines = v->lines.reserve(3 * table);
         for (int k = 0; k < 3; ++k) v->fl.p[k] = g2s[k]->is_inf() ? nullptr : lines + k * table;
         dev::verify_lines_kernel<<<1, 32, 0, v->stream>>>(v->g2.p, lines);
-        VCHECK_LAUNCH(1);
-        dev::verify_alphabeta_kernel<<<1, 32, 0, v->stream>>>(v->alpha.p, v->fl, v->e_ab.get(384));
-        VCHECK_LAUNCH(1);
-        VCUDA(cudaStreamSynchronize(v->stream));
+        ZKE_COUNT_LAUNCH(1); CHECK_LAUNCH();
+        dev::verify_alphabeta_kernel<<<1, 32, 0, v->stream>>>(v->alpha.p, v->fl, v->e_ab.reserve(384));
+        ZKE_COUNT_LAUNCH(1); CHECK_LAUNCH();
+        CUDA_OK(cudaStreamSynchronize(v->stream));
         return v.release();
     } catch (const std::exception& e) { set_err(err, errcap, e.what()); return nullptr; }
 }
@@ -368,17 +321,12 @@ int zke_verifier_batch(zke_verifier* v, size_t n, const uint8_t* proofs, const u
         const uint32_t np = v->n_public;
         if (!proofs || (np && !publics)) throw std::runtime_error("null argument");
         if (n > (size_t)1 << 26) throw std::runtime_error("batch too large");
-        VCUDA(cudaSetDevice(v->device));
+        CUDA_OK(cudaSetDevice(v->device));
         cudaStream_t st = v->stream;
         // weights: 128 bits, a zero weight replaced by 1 (as zke_verify_batch_json)
         std::vector<uint8_t> rnd(32 * n, 0), r16(16 * n);
         if (rand16) memcpy(r16.data(), rand16, 16 * n);
-        else {
-            FILE* fp = fopen("/dev/urandom", "rb");
-            const bool got = fp && fread(r16.data(), 1, r16.size(), fp) == r16.size();
-            if (fp) fclose(fp);
-            if (!got) throw std::runtime_error("cannot read /dev/urandom");
-        }
+        else random_bytes(r16.data(), r16.size());
         for (size_t i = 0; i < n; ++i) {
             memcpy(&rnd[32 * i], &r16[16 * i], 16);
             bool zero = true;
@@ -386,65 +334,65 @@ int zke_verifier_batch(zke_verifier* v, size_t n, const uint8_t* proofs, const u
             if (zero) rnd[32 * i] = 1;
         }
         const uint32_t nn = (uint32_t)n;
-        uint8_t* d_proofs = v->proofs.get(256 * n);
-        uint8_t* d_pub = v->publics.get(32 * n * (np ? np : 1));
-        uint8_t* d_rand = v->rand32.get(32 * n);
-        uint8_t* d_mont = v->mont.get(256 * n);
-        uint8_t* d_valid = v->valid.get(n);
-        VCUDA(cudaMemcpyAsync(d_proofs, proofs, 256 * n, cudaMemcpyHostToDevice, st));
-        if (np) VCUDA(cudaMemcpyAsync(d_pub, publics, 32 * n * np, cudaMemcpyHostToDevice, st));
-        VCUDA(cudaMemcpyAsync(d_rand, rnd.data(), 32 * n, cudaMemcpyHostToDevice, st));
+        uint8_t* d_proofs = v->proofs.reserve(256 * n);
+        uint8_t* d_pub = v->publics.reserve(32 * n * (np ? np : 1));
+        uint8_t* d_rand = v->rand32.reserve(32 * n);
+        uint8_t* d_mont = v->mont.reserve(256 * n);
+        uint8_t* d_valid = v->valid.reserve(n);
+        CUDA_OK(cudaMemcpyAsync(d_proofs, proofs, 256 * n, cudaMemcpyHostToDevice, st));
+        if (np) CUDA_OK(cudaMemcpyAsync(d_pub, publics, 32 * n * np, cudaMemcpyHostToDevice, st));
+        CUDA_OK(cudaMemcpyAsync(d_rand, rnd.data(), 32 * n, cudaMemcpyHostToDevice, st));
         dev::verify_validate_kernel<<<blocks(n), dev::VERIFY_THREADS, 0, st>>>(d_proofs, d_pub, nn, np, d_mont, d_valid);
-        VCHECK_LAUNCH(1);
+        ZKE_COUNT_LAUNCH(1); CHECK_LAUNCH();
         std::vector<uint8_t> valid(n);
-        VCUDA(cudaMemcpyAsync(valid.data(), d_valid, n, cudaMemcpyDeviceToHost, st));
-        VCUDA(cudaStreamSynchronize(st));
+        CUDA_OK(cudaMemcpyAsync(valid.data(), d_valid, n, cudaMemcpyDeviceToHost, st));
+        CUDA_OK(cudaStreamSynchronize(st));
         bool all_valid = true;
         for (size_t i = 0; i < n; ++i) all_valid = all_valid && valid[i];
 
         if (all_valid) {
-            uint8_t* d_nra = v->neg_ra.get(64 * n);
-            uint8_t* d_rc = v->rc.get(128 * n);
+            uint8_t* d_nra = v->neg_ra.reserve(64 * n);
+            uint8_t* d_rc = v->rc.reserve(128 * n);
             dev::verify_weight_kernel<<<blocks(n), dev::VERIFY_THREADS, 0, st>>>(d_mont, d_rand, nn, d_nra, d_rc);
-            VCHECK_LAUNCH(1);
+            ZKE_COUNT_LAUNCH(1); CHECK_LAUNCH();
             const size_t w = np + 1;
-            uint8_t* d_terms = v->terms.get(32 * w * n);
+            uint8_t* d_terms = v->terms.reserve(32 * w * n);
             dev::verify_coeff_terms_kernel<<<blocks(n), dev::VERIFY_THREADS, 0, st>>>(d_rand, d_pub, nn, np, d_terms);
-            VCHECK_LAUNCH(1);
-            const uint8_t* coeff = fold_all<dev::FrSumOp>(d_terms, nn, (uint32_t)w, v->terms_s0.get(32 * w * fold_scratch(n)),
-                                                          v->terms_s1.get(32 * w * fold_scratch(n)), st);
-            const uint8_t* csum = fold_all<dev::G1SumOp>(d_rc, nn, 1, v->rc_s0.get(128 * fold_scratch(n)),
-                                                         v->rc_s1.get(128 * fold_scratch(n)), st);
-            uint8_t* d_prod = v->products.get(128 * (np + 2));
+            ZKE_COUNT_LAUNCH(1); CHECK_LAUNCH();
+            const uint8_t* coeff = fold_all<dev::FrSumOp>(d_terms, nn, (uint32_t)w, v->terms_s0.reserve(32 * w * fold_scratch(n)),
+                                                          v->terms_s1.reserve(32 * w * fold_scratch(n)), st);
+            const uint8_t* csum = fold_all<dev::G1SumOp>(d_rc, nn, 1, v->rc_s0.reserve(128 * fold_scratch(n)),
+                                                         v->rc_s1.reserve(128 * fold_scratch(n)), st);
+            uint8_t* d_prod = v->products.reserve(128 * (np + 2));
             dev::verify_ic_mul_kernel<<<blocks(np + 2), dev::VERIFY_THREADS, 0, st>>>(coeff, v->ic.p, v->alpha.p, np, d_prod);
-            VCHECK_LAUNCH(1);
-            uint8_t* d_fixed = v->fixed_p.get(192);
+            ZKE_COUNT_LAUNCH(1); CHECK_LAUNCH();
+            uint8_t* d_fixed = v->fixed_p.reserve(192);
             dev::verify_fixed_points_kernel<<<1, 32, 0, st>>>(d_prod, np, csum, d_fixed);
-            VCHECK_LAUNCH(1);
-            uint8_t* d_f = v->f.get(384 * (n + 3));
+            ZKE_COUNT_LAUNCH(1); CHECK_LAUNCH();
+            uint8_t* d_f = v->f.reserve(384 * (n + 3));
             dev::verify_miller_kernel<<<blocks(n + 3), dev::VERIFY_THREADS, 0, st>>>(d_mont, d_nra, nn, v->fl, d_fixed, d_f);
-            VCHECK_LAUNCH(1);
-            const uint8_t* prod = fold_all<dev::F12ProdOp>(d_f, nn + 3, 1, v->f_s0.get(384 * fold_scratch(n + 3)),
-                                                           v->f_s1.get(384 * fold_scratch(n + 3)), st);
-            uint8_t* d_flag = v->flag.get(1);
+            ZKE_COUNT_LAUNCH(1); CHECK_LAUNCH();
+            const uint8_t* prod = fold_all<dev::F12ProdOp>(d_f, nn + 3, 1, v->f_s0.reserve(384 * fold_scratch(n + 3)),
+                                                           v->f_s1.reserve(384 * fold_scratch(n + 3)), st);
+            uint8_t* d_flag = v->flag.reserve(1);
             dev::verify_final_kernel<<<1, 32, 0, st>>>(prod, d_flag);
-            VCHECK_LAUNCH(1);
+            ZKE_COUNT_LAUNCH(1); CHECK_LAUNCH();
             uint8_t flag = 0;
-            VCUDA(cudaMemcpyAsync(&flag, d_flag, 1, cudaMemcpyDeviceToHost, st));
-            VCUDA(cudaStreamSynchronize(st));
+            CUDA_OK(cudaMemcpyAsync(&flag, d_flag, 1, cudaMemcpyDeviceToHost, st));
+            CUDA_OK(cudaStreamSynchronize(st));
             if (flag) {
                 if (ok) memset(ok, 1, n);
                 return (int)n;
             }
         }
         // per-proof verdicts
-        uint8_t* d_ok = v->ok.get(n);
+        uint8_t* d_ok = v->ok.reserve(n);
         dev::verify_single_kernel<<<blocks(n), dev::VERIFY_THREADS, 0, st>>>(d_mont, d_pub, d_valid, nn, np, v->ic.p, v->fl,
                                                                             v->e_ab.p, d_ok);
-        VCHECK_LAUNCH(1);
+        ZKE_COUNT_LAUNCH(1); CHECK_LAUNCH();
         std::vector<uint8_t> res(n);
-        VCUDA(cudaMemcpyAsync(res.data(), d_ok, n, cudaMemcpyDeviceToHost, st));
-        VCUDA(cudaStreamSynchronize(st));
+        CUDA_OK(cudaMemcpyAsync(res.data(), d_ok, n, cudaMemcpyDeviceToHost, st));
+        CUDA_OK(cudaStreamSynchronize(st));
         int count = 0;
         for (size_t i = 0; i < n; ++i) {
             if (ok) ok[i] = res[i];
@@ -468,14 +416,14 @@ int zke_selftest_pairing_gpu(int device, size_t n, const uint8_t* g1, const uint
             const G2AffineH q{Fq2{fq_at(g2 + 128 * i), fq_at(g2 + 128 * i + 32)}, Fq2{fq_at(g2 + 128 * i + 64), fq_at(g2 + 128 * i + 96)}};
             if (!g1_on_curve(p) || !g2_on_curve(q)) throw std::runtime_error("point " + std::to_string(i) + " is not on its curve");
         }
-        use_device(device);
-        DevMem d1, d2, d3;
-        VCUDA(cudaMemcpy(d1.get(64 * n), g1, 64 * n, cudaMemcpyHostToDevice));
-        VCUDA(cudaMemcpy(d2.get(128 * n), g2, 128 * n, cudaMemcpyHostToDevice));
-        dev::pairing_selftest_kernel<<<blocks(n), dev::VERIFY_THREADS>>>(d1.p, d2.p, (uint32_t)n, d3.get(384 * n));
-        VCHECK_LAUNCH(1);
-        VCUDA(cudaDeviceSynchronize());
-        VCUDA(cudaMemcpy(out, d3.p, 384 * n, cudaMemcpyDeviceToHost));
+        select_device(device);
+        DevBuf d1, d2, d3;
+        CUDA_OK(cudaMemcpy(d1.reserve(64 * n), g1, 64 * n, cudaMemcpyHostToDevice));
+        CUDA_OK(cudaMemcpy(d2.reserve(128 * n), g2, 128 * n, cudaMemcpyHostToDevice));
+        dev::pairing_selftest_kernel<<<blocks(n), dev::VERIFY_THREADS>>>(d1.p, d2.p, (uint32_t)n, d3.reserve(384 * n));
+        ZKE_COUNT_LAUNCH(1); CHECK_LAUNCH();
+        CUDA_OK(cudaDeviceSynchronize());
+        CUDA_OK(cudaMemcpy(out, d3.p, 384 * n, cudaMemcpyDeviceToHost));
         return 0;
     } catch (const std::exception& e) { set_err(err, errcap, e.what()); return -1; }
 }
