@@ -51,6 +51,16 @@ zke_circuit* zke_circuit_build(const char* template_name, const int64_t* params,
 zke_circuit* zke_circuit_build_regex(const char* const* parts, const uint8_t* is_public, size_t n_parts, uint32_t msg_len,
                                      char* err, size_t errcap);
 void zke_circuit_free(zke_circuit* c);
+/* circom's constraint system: an iden3 `.r1cs` image (what `circom --r1cs` writes and `snarkjs r1cs info` / `snarkjs groth16
+ * setup` read, /root/reference/docs/zk-email-docs/UsageGuide/README.md steps 3-5; layout in r1cs.cpp), BN254 only.  The
+ * circuit holds the constraints in file order (duplicate wires and zero coefficients kept) and no witness program:
+ * zke_witness, zke_fullprove, zke_fullprove_submit, zke_upload_inputs, zke_pack_inputs_json and zke_fullprove_json refuse
+ * it, witnesses come in through zke_load_witness / zke_wtns_prove.  Key setup, contributions, key checks and proving take
+ * it like any other circuit.  The image may be a memory-mapped file; nothing of it is kept. */
+zke_circuit* zke_circuit_from_r1cs(const void* r1cs, size_t len, char* err, size_t errcap);
+/* The circuit as an `.r1cs` image (sections 1, 2, 3; the labels read with the circuit, else the identity map).  out == NULL:
+ * returns the size needed; -2 if cap is too small; < 0 on error. */
+int64_t zke_circuit_write_r1cs(const zke_circuit* c, uint8_t* out, size_t cap);
 
 typedef struct zke_circuit_info {
     uint32_t n_vars;        /* witness length m, w[0] = 1 */
@@ -190,7 +200,9 @@ int zke_ptau_verify(const void* ptau, size_t len, const void* prev, size_t prev_
  * One host thread per context (or external locking).  All calls are synchronous at the ABI.
  * ------------------------------------------------------------------------------------------------- */
 /* `c` may be NULL when the key was loaded from a `.zkey`: such a context proves externally computed witnesses
- * (zke_load_witness / zke_wtns_prove + zke_prove) from the key's own coefficient matrices. */
+ * (zke_load_witness / zke_wtns_prove + zke_prove) from the key's own coefficient matrices.  With a circuit read from an
+ * `.r1cs` and a key that carries coefficient matrices (loaded from a `.zkey`, or made by zke_zkey_from_ptau), the key's A and
+ * B must equal the circuit's as linear forms ("zkey does not belong to this circuit: A row i differs" otherwise). */
 zke_ctx* zke_ctx_open(const zke_circuit* c, const zke_zkey* zkey_or_null, int device, uint32_t max_batch,
                       char* err, size_t errcap);
 void zke_ctx_close(zke_ctx* x);
@@ -227,6 +239,11 @@ int zke_witness(zke_ctx* x, const uint8_t* inputs, size_t batch, uint8_t* wtns_o
                 char* err, size_t errcap);
 /* Makes host witnesses resident (snarkjs `groth16 prove zkey wtns` entry). */
 int zke_load_witness(zke_ctx* x, const uint8_t* wtns, size_t batch, char* err, size_t errcap);
+/* `snarkjs wtns check` (/root/reference/docs/zk-email-docs/UsageGuide/README.md step 6) for the first `batch` witnesses made
+ * resident by zke_load_witness (or zke_witness): every constraint of the circuit, one kernel launch.  Needs the circuit (a
+ * context opened from a `.zkey` alone has no C matrix); works without a key.  status (optional) and the return value as for
+ * zke_witness: the number of failing witnesses, per witness -1 or the first violated constraint ("Assert Failed: ..."). */
+int zke_check_witness(zke_ctx* x, size_t batch, int32_t* status, char* err, size_t errcap);
 /* Groth16 prove for the resident witnesses (snarkjs.groth16.prove).  rs (optional): [batch][2][32] fixed blinding
  * scalars r, s (parity tests); NULL draws them from /dev/urandom.  proofs_out: [batch][8][32] =
  * A.x, A.y, B.x.c0, B.x.c1, B.y.c0, B.y.c1, C.x, C.y (standard form, LE).  publics_out: [batch][n_public][32]. */

@@ -356,6 +356,7 @@ int zke_pack_inputs_json(const zke_circuit* c, const char* input_json, uint8_t* 
     try {
         if (!c || !input_json || !out) throw std::runtime_error("null argument");
         const Circuit& k = c->c;
+        if (k.r1cs_only) throw std::runtime_error(R1CS_NO_PROGRAM);
         const size_t n_in = k.n_inputs();
         if (cap < 32 * n_in) throw std::runtime_error("output buffer too small");
         JV in = JParser(input_json).parse();
@@ -382,6 +383,7 @@ int zke_fullprove_json(zke_ctx* x, const zke_circuit* c, const char* input_json,
     try {
         if (!x || !c) throw std::runtime_error("null argument");
         const Circuit& k = c->c;
+        if (k.r1cs_only) throw std::runtime_error(R1CS_NO_PROGRAM);
         std::vector<uint8_t> packed(32 * (size_t)std::max(1u, k.n_inputs()));
         int rc = zke_pack_inputs_json(c, input_json, packed.data(), packed.size(), err, errcap);
         if (rc) return rc;

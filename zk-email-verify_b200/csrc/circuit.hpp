@@ -157,6 +157,13 @@ struct Circuit {
     // (built by finalize; ZKE_ARR_REGEX_SEEDS); the engine appends the same image to the program's aux table
     std::vector<uint32_t> regex_flat;
 
+    // Read from an iden3 `.r1cs` (r1cs.cpp): the constraint system alone.  The witness program above is empty, witnesses
+    // come from elsewhere (circom's witness calculator); nLabels and the section-3 wire -> label map are kept so that the
+    // file can be written back as it came (labels empty: the identity map, as for builder circuits).
+    bool r1cs_only = false;
+    uint64_t n_labels = 0;
+    std::vector<uint64_t> labels;
+
     uint32_t n_levels() const { return level_ptr.empty() ? 0 : (uint32_t)level_ptr.size() - 1; }
     const SignalGroup* find_group(const std::string& n) const;
     uint32_t domain_log2() const;  // smallest k with 2^k >= n_constraints + n_public + 1

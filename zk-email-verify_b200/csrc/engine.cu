@@ -19,6 +19,7 @@ cudaError_t upload_constants_verify(const FieldConsts*, const FieldConsts*);
 #include "../../include/zkemail_b200.h"
 #include "cuda_host.hpp"
 #include "engine.hpp"
+#include "binfile.hpp"
 #include "ec_host.hpp"
 #include "setup_host.hpp"
 #include <algorithm>
@@ -310,40 +311,6 @@ static zke_zkey* do_setup(const zke_circuit* zc, uint64_t seed, int device) {
 // the raw witness in Montgomery arithmetic twice).  The formats live in the un-vendored @iden3/binfileutils /
 // snarkjs 0.5.0 (SURVEY 8(b)); the call sites are chunked-zkey.ts:80-84 and UsageGuide/README.md:139-195.
 namespace {
-struct SecView { const uint8_t* p = nullptr; size_t n = 0; };
-struct BinSection { uint32_t type; SecView view; };
-
-uint32_t rd32(const uint8_t* p) { uint32_t v; memcpy(&v, p, 4); return v; }
-uint64_t rd64(const uint8_t* p) { uint64_t v; memcpy(&v, p, 8); return v; }
-
-// The sections of a container of len >= 12 bytes, in file order.  The caller checks the magic and the version first,
-// and the section types and contents after; `file` (".zkey", ...) names the format in the truncation errors.
-std::vector<BinSection> binfile_sections(const uint8_t* b, size_t len, const char* file) {
-    std::vector<BinSection> out;
-    const uint32_t n_sec = rd32(b + 8);
-    size_t pos = 12;
-    for (uint32_t i = 0; i < n_sec; ++i) {
-        if (len - pos < 12) throw std::runtime_error(std::string("truncated ") + file + " (section header)");
-        const uint32_t type = rd32(b + pos);
-        const uint64_t size = rd64(b + pos + 4);
-        pos += 12;
-        if (size > len - pos) throw std::runtime_error(std::string("truncated ") + file + " (section " + std::to_string(type) + ")");
-        out.push_back(BinSection{type, SecView{b + pos, (size_t)size}});
-        pos += (size_t)size;
-    }
-    return out;
-}
-
-// appends iden3 binfile pieces to a caller buffer
-struct BinWriter {
-    uint8_t* p;
-    void u32(uint32_t v) { memcpy(p, &v, 4); p += 4; }
-    void u64(uint64_t v) { memcpy(p, &v, 8); p += 8; }
-    void bytes(const void* src, size_t n) { memcpy(p, src, n); p += n; }
-    void header(const char* magic, uint32_t version, uint32_t n_sections) { bytes(magic, 4); u32(version); u32(n_sections); }
-    void section(int s, size_t size) { u32((uint32_t)s); u64(size); }
-};
-
 void split_container(const uint8_t* b, size_t len, SecView sec[11]) {
     if (!b || len < 12 || memcmp(b, "zkey", 4) != 0) throw std::runtime_error("not a .zkey file (bad magic)");
     if (rd32(b + 4) != 1) throw std::runtime_error("unsupported .zkey version");
@@ -571,6 +538,51 @@ static void alloc_slot(zke_ctx* x, zke_ctx::Slot& S) {
     S.allocated = true;
 }
 
+// The key's A and B (`.zkey` section 4 form: CSR over the 2^log_n domain rows) against the circuit's, compared as linear
+// forms: a row's terms sorted by signal, duplicates added, zero terms dropped.  Rows of the circuit, then the n_public + 1
+// extra rows of A (1 * w_j), then nothing.  Rows whose terms are listed identically are compared without the sort.
+static void check_key_matrices(const Circuit& c, const zke_zkey& zk) {
+    const size_t N = (size_t)1 << zk.log_n;
+    const uint32_t nc = c.n_constraints, l = c.n_public();
+    typedef std::vector<std::pair<uint32_t, Fr>> Form;
+    auto canonical = [](Form& f) {
+        std::sort(f.begin(), f.end(), [](const std::pair<uint32_t, Fr>& a, const std::pair<uint32_t, Fr>& b) { return a.first < b.first; });
+        size_t o = 0;
+        for (size_t i = 0; i < f.size();) {
+            std::pair<uint32_t, Fr> t = f[i++];
+            while (i < f.size() && f[i].first == t.first) t.second = t.second + f[i++].second;
+            if (!t.second.is_zero()) f[o++] = t;
+        }
+        f.resize(o);
+    };
+    Form x, y;
+    auto compare = [&](const char* name, const std::vector<uint32_t>& kp, const std::vector<uint32_t>& kv, const std::vector<uint32_t>& kc,
+                       const std::vector<uint32_t>& cp, const std::vector<uint32_t>& cv, const std::vector<uint32_t>& cc, bool extra) {
+        for (size_t row = 0; row < N; ++row) {
+            const uint32_t kb = kp[row], ke = kp[row + 1];
+            if (row < nc) {
+                const uint32_t b = cp[row], e = cp[row + 1];
+                bool same = e - b == ke - kb;
+                for (uint32_t k = 0; same && k < e - b; ++k) same = cv[b + k] == kv[kb + k] && c.coefs[cc[b + k]] == zk.coefs[kc[kb + k]];
+                if (same) continue;
+            }
+            x.clear(); y.clear();
+            for (uint32_t k = kb; k < ke; ++k) x.emplace_back(kv[k], Fr::from_u256(zk.coefs[kc[k]]));
+            if (row < nc) {
+                for (uint32_t k = cp[row]; k < cp[row + 1]; ++k) y.emplace_back(cv[k], Fr::from_u256(c.coefs[cc[k]]));
+            } else if (extra && row <= (size_t)nc + l) {
+                y.emplace_back((uint32_t)(row - nc), Fr::one());
+            }
+            canonical(x); canonical(y);
+            bool same = x.size() == y.size();
+            for (size_t i = 0; same && i < x.size(); ++i) same = x[i].first == y[i].first && x[i].second == y[i].second;
+            if (!same) throw std::runtime_error(std::string("zkey does not belong to this circuit: ") + name + " row " + std::to_string(row) + " differs");
+        }
+    };
+    compare("A", zk.a_ptr, zk.a_var, zk.a_coef, c.a_ptr, c.a_var, c.a_coef, true);
+    compare("B", zk.b_ptr, zk.b_var, zk.b_coef, c.b_ptr, c.b_var, c.b_coef, false);
+}
+
 static zke_ctx* do_open(const zke_circuit* zc, const zke_zkey* zk, int device, uint32_t max_batch) {
     select_device(device);
     const Circuit* cp = zc ? &zc->c : nullptr;
@@ -616,8 +628,11 @@ static zke_ctx* do_open(const zke_circuit* zc, const zke_zkey* zk, int device, u
         x->coef_r.upload(cr);
     }
 
-    // witness program
-    if (cp) {
+    // a circuit read from an `.r1cs` and a key that carries its own coefficient matrices: they must be the same system
+    if (zk && cp && cp->r1cs_only && zk->has_coefs) check_key_matrices(*cp, *zk);
+
+    // witness program (none for a circuit read from an `.r1cs`: its witnesses are loaded)
+    if (cp && !cp->r1cs_only) {
         const Circuit& c = *cp;
         // Streamed witness program (device_engine.cuh): per level, ops sorted by kind / size so that the threads of an
         // iteration do similar work, padded with no-ops to whole iterations of WITNESS_THREADS records; the LC terms
@@ -1017,6 +1032,7 @@ static void require_idle(const zke_ctx* x) {
 static void do_witness(zke_ctx* x, zke_ctx::Slot& S, const uint8_t* inputs, size_t batch) {
     if (!x->circuit) throw std::runtime_error("this context was opened from a .zkey alone: it has no witness program (use zke_load_witness / zke_wtns_prove)");
     const Circuit& c = x->circuit->c;
+    if (c.r1cs_only) throw std::runtime_error(R1CS_NO_PROGRAM);
     if (batch == 0 || batch > x->max_batch) throw std::runtime_error("batch exceeds the context's max_batch");
     CUDA_OK(cudaSetDevice(x->device));
     const uint8_t* in_dev = x->inputs.p;
@@ -1574,6 +1590,7 @@ void zke_ctx_close(zke_ctx* x) {
 int zke_upload_inputs(zke_ctx* x, const uint8_t* inputs, size_t batch, char* err, size_t errcap) {
     try {
         if (!x || !inputs) throw std::runtime_error("null argument");
+        if (x->circuit && x->circuit->c.r1cs_only) throw std::runtime_error(R1CS_NO_PROGRAM);
         if (batch == 0 || batch > x->max_batch) throw std::runtime_error("batch exceeds the context's max_batch");
         require_idle(x);
         CUDA_OK(cudaSetDevice(x->device));
@@ -1625,6 +1642,21 @@ int zke_load_witness(zke_ctx* x, const uint8_t* wtns, size_t batch, char* err, s
         if (!x || !wtns) throw std::runtime_error("null argument");
         require_idle(x);
         load_witness(x, x->slots[0], wtns, batch);
+        return 0;
+    } catch (const std::exception& e) { set_err(err, errcap, e.what()); return -1; }
+}
+
+int zke_check_witness(zke_ctx* x, size_t batch, int32_t* status, char* err, size_t errcap) {
+    try {
+        if (!x) throw std::runtime_error("null context");
+        if (!x->circuit) throw std::runtime_error("this context was opened from a .zkey alone: it has no C matrix to check witnesses against (open it with the circuit)");
+        require_idle(x);
+        zke_ctx::Slot& S = x->slots[0];
+        if (batch == 0 || batch > S.loaded) throw std::runtime_error("no witness loaded for this batch (call zke_load_witness first)");
+        CUDA_OK(cudaSetDevice(x->device));
+        std::string msg;
+        int bad = do_check(x, S, batch, status, msg);
+        if (bad) { set_err(err, errcap, msg); return bad; }
         return 0;
     } catch (const std::exception& e) { set_err(err, errcap, e.what()); return -1; }
 }

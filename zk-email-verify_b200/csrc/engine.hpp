@@ -7,6 +7,9 @@ namespace zke {
 void set_err(char* err, size_t cap, const std::string& msg);
 void random_bytes(void* out, size_t n);   // from /dev/urandom
 void random_scalar(U256& out);   // uniform in [0, r), from /dev/urandom
+// the refusal of every entry point that needs a witness program, for a circuit read from an `.r1cs`
+constexpr const char* R1CS_NO_PROGRAM =
+    "this circuit was read from an .r1cs: it has no witness program (load witnesses with zke_load_witness / zke_wtns_prove)";
 }
 
 struct zke_circuit {

@@ -1,6 +1,6 @@
 """H100-native host package mirroring the @zk-email/helpers surface for the EmailVerifier path
 (/root/reference/packages/helpers/src/index.ts:1-4)."""
-from .circuit import Circuit, FR_MODULUS  # noqa: F401
+from .circuit import Circuit, FR_MODULUS, r1cs_info  # noqa: F401
 from .constants import *  # noqa: F401,F403
 from .binary_format import (bigint_to_chunked_bytes, bytes_to_bigint, int64_to_bytes, int8_to_bytes,  # noqa: F401
                             to_circom_bigint_bytes, uint8array_to_char_array)

@@ -39,6 +39,8 @@ def _sig(name, restype, argtypes):
 
 zke_circuit_build = _sig("zke_circuit_build", c_void_p, [c_char_p, ctypes.POINTER(c_i64), c_size_t, c_char_p, c_size_t])
 zke_circuit_free = _sig("zke_circuit_free", None, [c_void_p])
+zke_circuit_from_r1cs = _sig("zke_circuit_from_r1cs", c_void_p, [c_void_p, c_size_t, c_char_p, c_size_t])
+zke_circuit_write_r1cs = _sig("zke_circuit_write_r1cs", c_i64, [c_void_p, c_void_p, c_size_t])
 zke_circuit_get_info = _sig("zke_circuit_get_info", c_int, [c_void_p, ctypes.POINTER(CircuitInfo)])
 zke_circuit_group = _sig("zke_circuit_group", c_int, [c_void_p, c_u32, c_char_p, c_size_t, ctypes.POINTER(c_u32),
                                                        ctypes.POINTER(c_u32), ctypes.POINTER(c_int)])
@@ -80,6 +82,7 @@ zke_ctx_stream = _sig("zke_ctx_stream", c_void_p, [c_void_p])
 zke_kernel_launches = _sig("zke_kernel_launches", c_u64, [])
 zke_witness = _sig("zke_witness", c_int, [c_void_p, c_void_p, c_size_t, c_void_p, c_void_p, c_char_p, c_size_t])
 zke_load_witness = _sig("zke_load_witness", c_int, [c_void_p, c_void_p, c_size_t, c_char_p, c_size_t])
+zke_check_witness = _sig("zke_check_witness", c_int, [c_void_p, c_size_t, c_void_p, c_char_p, c_size_t])
 zke_prove = _sig("zke_prove", c_int, [c_void_p, c_size_t, c_void_p, c_void_p, c_void_p, c_void_p, c_char_p, c_size_t])
 zke_fullprove = _sig("zke_fullprove", c_int, [c_void_p, c_void_p, c_size_t, c_void_p, c_void_p, c_void_p, c_void_p, c_char_p, c_size_t])
 zke_verify_json = _sig("zke_verify_json", c_int, [c_char_p, c_char_p, c_char_p, c_char_p, c_size_t])

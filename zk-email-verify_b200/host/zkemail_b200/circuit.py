@@ -3,8 +3,11 @@
 from __future__ import annotations
 import ctypes
 from . import _lib as L
+from ._mapped import mapped_buffer
 
 FR_MODULUS = 21888242871839275222246405745257275088548364400416034343698204186575808495617
+R1CS_NO_PROGRAM = ("this circuit was read from an .r1cs: it has no witness program "
+                   "(load witnesses with zke_load_witness / zke_wtns_prove)")
 
 
 class Circuit:
@@ -39,6 +42,29 @@ class Circuit:
             raise L.ZkeError(err.value.decode())
         return cls("Regex", (msg_len,), _handle=h)
 
+    @classmethod
+    def from_r1cs(cls, src):
+        """circom's constraint system: an iden3 `.r1cs` (bytes, a buffer or a path, which is memory-mapped), as `circom
+        --r1cs` writes it for `snarkjs groth16 setup`.  The circuit has no witness program: its witnesses come from circom's
+        witness calculator (Context.load_witness / wtns_prove), and key setup, contributions and proving work as usual."""
+        err = ctypes.create_string_buffer(L.ERRCAP)
+        with mapped_buffer(src) as (ptr, n):
+            h = L.zke_circuit_from_r1cs(ptr, n, err, L.ERRCAP)
+        if not h:
+            raise L.ZkeError(err.value.decode())
+        return cls("r1cs", (), _handle=h)
+
+    def write_r1cs(self) -> bytes:
+        """The constraint system as an `.r1cs` image, written natively: the bytes of iden3_binfile.write_r1cs, and for a
+        circuit read with from_r1cs its labels and constraints as they were read."""
+        n = L.zke_circuit_write_r1cs(self._h, None, 0)
+        if n < 0:
+            raise L.ZkeError("r1cs export failed")
+        buf = ctypes.create_string_buffer(n)
+        if L.zke_circuit_write_r1cs(self._h, buf, n) != n:
+            raise L.ZkeError("r1cs export failed")
+        return buf.raw
+
     def __del__(self):
         if getattr(self, "_h", None):
             L.zke_circuit_free(self._h)
@@ -56,6 +82,8 @@ class Circuit:
         """snarkjs input JSON ({name: decimal string | number | list}) -> [n_inputs][32] little-endian bytes,
         in witness order.  Mirrors the checks of circom_runtime's witness calculator: every declared input
         must be present with the right number of values ("Not all inputs have been set" / "Too many values")."""
+        if self.template == "r1cs":
+            raise L.ZkeError(R1CS_NO_PROGRAM)
         base = 1 + self.info.n_outputs
         buf = bytearray(32 * self.n_inputs)
         seen = set()
@@ -84,6 +112,26 @@ class Circuit:
     def scope_name(self, idx: int) -> str:
         s = L.zke_circuit_scope_name(self._h, idx)
         return s.decode() if s else "?"
+
+
+def r1cs_info(src) -> dict:
+    """`snarkjs r1cs info`: the fields it prints for an `.r1cs` (bytes, a buffer or a path).  The whole file is read and
+    checked as Circuit.from_r1cs does; nLabels comes from its header."""
+    import struct
+    c = Circuit.from_r1cs(src)
+    with mapped_buffer(src) as (ptr, n):
+        view = (ctypes.c_char * n).from_address(ptr) if isinstance(ptr, int) else ptr
+        n_sec, pos, labels = struct.unpack_from("<I", view, 8)[0], 12, None
+        for _ in range(n_sec):
+            typ, size = struct.unpack_from("<IQ", view, pos)
+            if typ == 1:
+                labels = struct.unpack_from("<Q", view, pos + 12 + 4 + 32 + 16)[0]
+                break
+            pos += 12 + size
+        del view
+    i = c.info
+    return {"curve": "bn128", "wires": i.n_vars, "constraints": i.n_constraints, "private_inputs": i.n_prv_inputs,
+            "public_inputs": i.n_pub_inputs, "outputs": i.n_outputs, "labels": labels}
 
 
 def _flatten(v):

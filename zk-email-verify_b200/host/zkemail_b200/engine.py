@@ -3,6 +3,7 @@ from __future__ import annotations
 import ctypes
 import json
 from . import _lib as L
+from ._mapped import mapped_buffer
 from .circuit import Circuit
 
 
@@ -54,7 +55,7 @@ class Zkey:
         """`snarkjs groth16 setup` for this engine's R1CS: a key from a prepared phase-2 `.ptau` (bytes, a writable buffer or
         a path, which is memory-mapped).  gamma = delta = 1, so the key is a toy until `contribute` is applied."""
         err = ctypes.create_string_buffer(L.ERRCAP)
-        with _ptau_buffer(ptau) as (ptr, n):
+        with mapped_buffer(ptau) as (ptr, n):
             h = L.zke_zkey_from_ptau(circuit.handle, ptr, n, device, err, L.ERRCAP)
         if not h:
             raise L.ZkeError(err.value.decode())
@@ -140,36 +141,6 @@ class Zkey:
         return buf.raw
 
 
-class _ptau_buffer:
-    """(pointer, length) of a `.ptau` given as bytes, a buffer or a path; a path is memory-mapped copy-on-write (files for
-    large domains are several GB), so nothing is read that the library does not touch."""
-
-    def __init__(self, ptau):
-        self._src, self._mm, self._arr = ptau, None, None
-
-    def __enter__(self):
-        import mmap
-        import os
-        p = self._src
-        if isinstance(p, (str, os.PathLike)):
-            with open(p, "rb") as f:
-                self._mm = mmap.mmap(f.fileno(), 0, access=mmap.ACCESS_COPY)
-            p = self._mm
-        if isinstance(p, bytes):
-            return p, len(p)
-        with memoryview(p) as mv:
-            if mv.readonly:
-                return bytes(mv), mv.nbytes
-            n = mv.nbytes
-        self._arr = (ctypes.c_char * n).from_buffer(p)
-        return ctypes.addressof(self._arr), n
-
-    def __exit__(self, *exc):
-        self._arr = None
-        if self._mm is not None:
-            self._mm.close()
-        return False
-
 
 def ptau_info(ptau, circuit: Circuit | None = None) -> dict:
     """Structure of a prepared `.ptau` as the library reads it (host only): {"power", "sections": {type: (offset, size)}}.
@@ -177,7 +148,7 @@ def ptau_info(ptau, circuit: Circuit | None = None) -> dict:
     power = L.c_u32()
     offs, sizes = (L.c_u64 * 16)(), (L.c_u64 * 16)()
     err = ctypes.create_string_buffer(L.ERRCAP)
-    with _ptau_buffer(ptau) as (ptr, n):
+    with mapped_buffer(ptau) as (ptr, n):
         rc = L.zke_ptau_info(circuit.handle if circuit is not None else None, ptr, n, ctypes.byref(power), offs, sizes, err, L.ERRCAP)
     if rc != 0:
         raise L.ZkeError(err.value.decode())
@@ -228,14 +199,14 @@ def ptau_contribute(ptau, secrets: tuple | None = None, device: int = 0) -> tupl
     if tab is not None and len(tab) != 96:
         raise ValueError("secrets must be three integers below 2^256")
     receipt = ctypes.create_string_buffer(384)
-    with _ptau_buffer(ptau) as (ptr, n):
+    with mapped_buffer(ptau) as (ptr, n):
         out = _ptau_write(lambda o, cap, err: L.zke_ptau_contribute(ptr, n, tab, device, o, cap, receipt if o else None, err, L.ERRCAP))
     return out, receipt.raw
 
 
 def ptau_prepare(ptau, device: int = 0) -> bytearray:
     """`snarkjs powersoftau prepare phase2`: the unprepared `.ptau` plus its Lagrange sections 12-15, computed on the GPU."""
-    with _ptau_buffer(ptau) as (ptr, n):
+    with mapped_buffer(ptau) as (ptr, n):
         return _ptau_write(lambda out, cap, err: L.zke_ptau_prepare(ptr, n, device, out, cap, err, L.ERRCAP))
 
 
@@ -251,11 +222,11 @@ def ptau_report(ptau, prev=None, receipt: bytes | None = None, device: int = 0, 
     if rand is not None and len(rand) != 16:
         raise ValueError("rand must be 16 bytes")
     err = ctypes.create_string_buffer(L.ERRCAP)
-    with _ptau_buffer(ptau) as (ptr, n):
+    with mapped_buffer(ptau) as (ptr, n):
         if prev is None:
             rc = L.zke_ptau_verify(ptr, n, None, 0, None, bytes(rand) if rand is not None else None, device, err, L.ERRCAP)
         else:
-            with _ptau_buffer(prev) as (pptr, pn):
+            with mapped_buffer(prev) as (pptr, pn):
                 rc = L.zke_ptau_verify(ptr, n, pptr, pn, bytes(receipt), bytes(rand) if rand is not None else None, device, err, L.ERRCAP)
     if rc < 0:
         raise L.ZkeError(err.value.decode())
@@ -331,6 +302,28 @@ class Context:
         err = ctypes.create_string_buffer(L.ERRCAP)
         if L.zke_load_witness(self._h, wtns, batch, err, L.ERRCAP) != 0:
             raise L.ZkeError(err.value.decode())
+
+    def check_witness(self, batch: int, raise_on_fail: bool = True) -> list:
+        """`snarkjs wtns check` for the first `batch` witnesses of load_witness: per witness -1, or the first violated
+        constraint.  Raises AssertFailed ("Assert Failed: constraint i ...") when one fails, unless raise_on_fail is False."""
+        status = (ctypes.c_int32 * batch)()
+        err = ctypes.create_string_buffer(L.ERRCAP)
+        rc = L.zke_check_witness(self._h, batch, status, err, L.ERRCAP)
+        if rc < 0:
+            raise L.ZkeError(err.value.decode())
+        if rc > 0 and raise_on_fail:
+            raise AssertFailed(err.value.decode())
+        return list(status)
+
+    def check_wtns(self, wtns_file: bytes, raise_on_fail: bool = True) -> int:
+        """`snarkjs wtns check circuit.r1cs witness.wtns`: one `.wtns` file image against the circuit's constraints.  Returns
+        -1 when every constraint holds, else the first violated one (AssertFailed unless raise_on_fail is False)."""
+        from .iden3_binfile import read_wtns
+        data = read_wtns(bytes(wtns_file))
+        if len(data) != 32 * self.n_vars:
+            raise L.ZkeError(f".wtns has {len(data) // 32} values, the circuit has {self.n_vars} wires")
+        self.load_witness(data, 1)
+        return self.check_witness(1, raise_on_fail)[0]
 
     def _prove_call(self, fn, head_args, batch, rs, raise_on_fail):
         npub = self.n_public
