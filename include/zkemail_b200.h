@@ -107,6 +107,27 @@ enum {
 const void* zke_circuit_array(const zke_circuit* c, int which, size_t* n_elems);
 const char* zke_circuit_scope_name(const zke_circuit* c, uint32_t scope_index);
 
+/* What the engine's lowering of the witness program builds for this circuit (the stream the witness kernel walks: the native
+ * SHA-256 and regex-seeding substitutions, levels cut into iterations of 512 records and padded to rounds of `cluster`
+ * iterations), computed on the host - no device needed.  zke_ctx_open lowers with the same code; its options come from
+ * ZKE_NATIVE_SHA, ZKE_NATIVE_REGEX, ZKE_COOP_FPMUL (default 1 each) and ZKE_WITNESS_CLUSTER (default: chosen from max_batch).
+ * cluster: 1, 2, 4 or 8.  level_ops (optional, may be NULL): the first min(n_levels, level_cap) entries receive the number of
+ * records of each level that are not cooperative ops.  A circuit read from an `.r1cs` has no program: an error.
+ * Returns 0, or non-zero with a message in err. */
+typedef struct zke_program_stats {
+    uint32_t n_levels;      /* dependency depth after the substitutions */
+    uint32_t n_iters;       /* iterations of 512 records, padding iterations included */
+    uint32_t n_ops_kept;    /* records that are not cooperative ops (the sum of level_ops) */
+    uint32_t n_coop_ops;    /* cooperative ops: native SHA-256 blocks, regex seeds, FpMul hints */
+    uint32_t n_terms;       /* linear-combination terms of the stream, alignment padding included */
+    uint32_t cluster;
+    uint64_t digest;        /* 64-bit FNV-1a over the stream's five arrays (op records, iteration headers, terms, aux table,
+                               cooperative ops, in that order): per array its word count as 8 little-endian bytes, then its
+                               32-bit words as 4 little-endian bytes each */
+} zke_program_stats;
+int zke_circuit_program_stats(const zke_circuit* c, int native_sha, int native_regex, int coop_fpmul, uint32_t cluster,
+                              zke_program_stats* out, uint32_t* level_ops, size_t level_cap, char* err, size_t errcap);
+
 
 /* ---------------------------------------------------------------------------------------------------
  * Proving key.  zke_setup() is a TOY trusted setup (`snarkjs groth16 setup` role,

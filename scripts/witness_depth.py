@@ -1,95 +1,20 @@
-"""CPU-side analysis of the witness program the engine builds at open time (engine.cu: do_open): the native SHA-256 and
-regex-seeding substitutions are replayed on the exported program (ZKE_ARR_OPS / LC / AUX / SHA_BLOCKS / REGEX_SEEDS), the
-ops are levelised again, and the number of levels and of 512-op iterations is printed - what the level-synchronous
-witness kernel (witness.cu) walks.   python scripts/witness_depth.py [Template p1,p2,...]"""
-import ctypes, os, sys
+"""CPU-side analysis of the witness program the engine builds at open time (csrc/witness_program.cpp, reported by
+zke_circuit_program_stats): the number of levels and of 512-op iterations left after the native SHA-256 and regex-seeding
+substitutions - what the level-synchronous witness kernel (witness.cu) walks, here for one CTA per email.
+    python scripts/witness_depth.py [Template p1,p2,...]"""
+import os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "zk-email-verify_b200", "host"))
-import numpy as np
 import zkemail_b200 as z
-from zkemail_b200 import _lib as L
 
-OP_LIN, OP_QUAD, OP_SHRAND, OP_INVZ, OP_FPMUL, OP_SHRLC = 0, 1, 2, 3, 4, 5
 T = 512
 
 
-def arr(c, which, dtype=np.uint32):
-    n = L.c_size_t()
-    p = L.zke_circuit_array(c.handle, which, ctypes.byref(n))
-    if not n.value:
-        return np.zeros(0, dtype=dtype)
-    words = n.value * (5 if which == L.ARR_OPS else 1)          # ZKE_ARR_OPS counts 5-word records
-    return np.ctypeslib.as_array((ctypes.c_uint32 * words).from_address(p)).copy()
-
-
 def analyse(c, native_sha=True, native_rx=True):
-    ops = arr(c, L.ARR_OPS).reshape(-1, 5)
-    lc_ptr, lc_var, aux = arr(c, L.ARR_LC_PTR), arr(c, L.ARR_LC_VAR), arr(c, L.ARR_AUX)
-    sha, rx = arr(c, L.ARR_SHA_BLOCKS), arr(c, L.ARR_REGEX_SEEDS)
-    n_slots = int(max(ops[:, 1].max(), lc_var.max() if len(lc_var) else 0)) + 64
-    owner = np.full(n_slots + 1, -1, dtype=np.int64)
-    blocks, pos = [], 1
-    for bi in range(int(sha[0]) if len(sha) and native_sha else 0):
-        vb, ve, tb, te, nd = (int(x) for x in sha[pos:pos + 5]); pos += 5
-        inputs = sha[pos:pos + 768]; pos += 768 + 2 * nd
-        owner[vb:ve] = bi; owner[tb:te] = bi
-        blocks.append((vb, ve, [int(v) for v in inputs if v < 0xfffffffe]))
-    seeds, pos = [], 1
-    for _ in range(int(rx[0]) if len(rx) and native_rx else 0):
-        nd, nb, ns = (int(x) for x in rx[pos:pos + 3]); pos += 5
-        mode, ns = ns >> 31, ns & 0x7fffffff
-        byts = [int(v) for v in rx[pos:pos + nb]]; pos += nb + 64 * ns * (1 + mode)
-        seeds.append((byts, [int(v) for v in rx[pos:pos + 2 * nd:2]])); pos += 2 * nd
-    seeded = np.zeros(n_slots + 1, dtype=bool)
-    for _, vs in seeds:
-        seeded[vs] = True
-    level = np.zeros(n_slots + 1, dtype=np.int64)
-    def_pos = np.full(n_slots + 1, -1, dtype=np.int64)
-    for i, (code, dst, a, b_, c_) in enumerate(ops):
-        nd = 2 * int(aux[a + 1]) if code == OP_FPMUL else 1
-        def_pos[dst:dst + nd] = i
-    at = {}
-    for bi, (vb, ve, ins) in enumerate(blocks):
-        at.setdefault(max([def_pos[v] + 1 for v in ins] + [0]), []).append(("sha", bi))
-    for ri, (byts, vs) in enumerate(seeds):
-        at.setdefault(max([def_pos[v] + 1 for v in byts] + [0]), []).append(("rx", ri))
-    def lcl(i):
-        s, e = lc_ptr[i], lc_ptr[i + 1]
-        return int(level[lc_var[s:e]].max()) if e > s else 0
-    counts = {}
-    n_coop = {}
-    for i in range(len(ops) + 1):
-        for kind, k in at.get(i, []):
-            if kind == "sha":
-                vb, ve, ins = blocks[k]
-                l = (max(level[ins]) if ins else 0) + 1
-                level[vb:ve] = l
-            else:
-                byts, vs = seeds[k]
-                l = int(level[byts].max()) + 1
-                level[vs] = l
-            n_coop[l] = n_coop.get(l, 0) + 1
-        if i == len(ops):
-            break
-        code, dst, a, b_, c_ = (int(x) for x in ops[i])
-        if owner[dst] >= 0:
-            continue
-        if code in (OP_LIN, OP_SHRLC): l = lcl(a)
-        elif code == OP_QUAD: l = max(lcl(a), lcl(b_), lcl(c_))
-        elif code in (OP_SHRAND, OP_INVZ): l = int(level[a])
-        else:
-            kk = int(aux[a + 1]); l = int(level[aux[a + 2:a + 2 + 3 * kk]].max())
-        l += 1
-        if code == OP_FPMUL:
-            level[dst:dst + 2 * int(aux[a + 1])] = l
-            n_coop[l] = n_coop.get(l, 0) + 1
-        elif not seeded[dst]:
-            level[dst] = l
-        counts[l] = counts.get(l, 0) + (0 if code == OP_FPMUL else 1)
-    depth = max(list(counts) + list(n_coop))
-    iters = sum(max(1 if n_coop.get(l) else 0, -(-counts.get(l, 0) // T)) for l in range(1, depth + 1))
-    kept = sum(counts.values())
-    return depth, iters, kept, counts
+    """(levels, iterations, ops that are not cooperative ops, {level: such ops})"""
+    st = c.program_stats(native_sha=native_sha, native_regex=native_rx, cluster=1)
+    counts = {l + 1: n for l, n in enumerate(st["level_ops"])}
+    return st["n_levels"], st["n_iters"], st["n_ops_kept"], counts
 
 
 if __name__ == "__main__":

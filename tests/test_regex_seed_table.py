@@ -1,6 +1,6 @@
 """The state-seeding record of the zk-regex circuits (circuit.hpp: RegexSeed, ZKE_ARR_REGEX_SEEDS): the engine lets ONE
 automaton run per regex instance write every state signal, so that the per-position gadgets of all positions evaluate side
-by side instead of as a chain as long as the message (witness.cu: regex_coop, engine.cu: do_open).  Checked here on the CPU:
+by side instead of as a chain as long as the message (witness.cu: regex_coop, witness_program.cpp).  Checked here on the CPU:
 the oracle walks the ordinary witness program, and every recorded signal must hold bit `state` of the live-state set an
 independent Python run of the recorded transition table reaches at the recorded position - the values the device op writes.
 Role in the reference: the generated zk-regex templates (email-verifier.circom:5,126; un-vendored zk-regex-circom)."""

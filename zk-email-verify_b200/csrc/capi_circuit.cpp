@@ -4,6 +4,7 @@
 #include "gadgets.hpp"
 #include "bigdiv.hpp"
 #include "setup_host.hpp"
+#include "witness_program.hpp"
 #include <cstdio>
 #include <cstring>
 
@@ -360,6 +361,34 @@ const void* zke_circuit_array(const zke_circuit* c, int which, size_t* n) {
 const char* zke_circuit_scope_name(const zke_circuit* c, uint32_t i) {
     if (!c || i >= c->c.scopes.size()) return nullptr;
     return c->c.scopes[i].c_str();
+}
+
+int zke_circuit_program_stats(const zke_circuit* c, int native_sha, int native_regex, int coop_fpmul, uint32_t cluster,
+                              zke_program_stats* out, uint32_t* level_ops, size_t level_cap, char* err, size_t errcap) {
+    try {
+        if (!c || !out) throw std::runtime_error("null argument");
+        if (c->c.r1cs_only) throw std::runtime_error(R1CS_NO_PROGRAM);
+        if (cluster != 1 && cluster != 2 && cluster != 4 && cluster != 8) throw std::runtime_error("cluster must be 1, 2, 4 or 8");
+        LowerOptions opt;
+        opt.native_sha = native_sha != 0; opt.native_regex = native_regex != 0; opt.coop_fpmul = coop_fpmul != 0; opt.cluster = cluster;
+        const WitnessStream S = lower_witness_program(c->c, coef_words(c->c.coefs), opt);
+        memset(out, 0, sizeof *out);
+        out->n_levels = S.n_levels; out->n_iters = S.n_iters; out->cluster = S.cluster;
+        for (uint32_t n : S.level_ops) out->n_ops_kept += n;
+        for (uint32_t k = 0; k < S.n_iters; ++k) { out->n_coop_ops += S.iter_hdr[4 * k + 3] & 0x7fffffffu; out->n_terms += S.iter_info[3 * k + 2]; }
+        uint64_t h = 0xcbf29ce484222325ull;    // FNV-1a
+        auto eat = [&h](uint64_t v, int n_bytes) { for (int i = 0; i < n_bytes; ++i) { h ^= (v >> (8 * i)) & 0xff; h *= 0x100000001b3ull; } };
+        for (const std::vector<uint32_t>* a : {&S.ops, &S.iter_hdr, &S.terms, &S.aux, &S.coop}) {
+            eat(a->size(), 8);
+            for (uint32_t w : *a) eat(w, 4);
+        }
+        out->digest = h;
+        for (size_t l = 0; level_ops && l < S.level_ops.size() && l < level_cap; ++l) level_ops[l] = S.level_ops[l];
+        return 0;
+    } catch (const std::exception& e) {
+        set_err(err, errcap, e.what());
+        return -1;
+    }
 }
 
 int zke_selftest_fpmul_hint(uint32_t n, uint32_t k, const uint8_t* a, const uint8_t* b, const uint8_t* p, uint8_t* q, uint8_t* r) {

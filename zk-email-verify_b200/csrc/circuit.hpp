@@ -74,7 +74,7 @@ struct WOp {
 // creates is a bit of some 64-bit quantity of the compression (a sigma / Ch / Maj word, an AND of two rotations, one of
 // the adder sums), so a device can produce all of them from ONE native compression instead of walking the gadget's
 // ~320 dependency levels.  The witness program itself (Circuit::ops) is unchanged - the CPU oracle walks it - the
-// record only lets the engine substitute the sub-program (engine.cu: do_open).
+// record only lets the engine substitute the sub-program (witness_program.cpp).
 struct ShaBlock {
     uint32_t var_begin = 0, var_end = 0;      // signals created by the gadget: [var_begin, var_end), one descriptor each
     uint32_t temp_begin = 0, temp_end = 0;    // scratch slots created by the gadget (absolute slot numbers after finalize)
@@ -97,7 +97,7 @@ enum ShaQuantity : uint32_t {
 // of live DFA states per position is a plain automaton run, so a device can produce every state SIGNAL of the instance at
 // once ("seed" them) and the per-position gadgets (comparators, ANDs, ORs) of all positions then evaluate side by side.
 // The witness program keeps all of its ops - the seeded signals are simply written twice with the same value, and the
-// CPU oracle walks the program as it is (engine.cu: do_open uses the record when it levelises the program).
+// CPU oracle walks the program as it is (witness_program.cpp uses the record when it levelises the program).
 struct RegexSeed {
     uint32_t n_states = 0;            // <= 64
     std::vector<uint32_t> bytes;      // the variable holding message byte j (position j + 1 of the circuit; position 0 is the marker)

@@ -1,13 +1,15 @@
 // Device-side data structures and kernel launchers shared by the .cu files.
 #pragma once
 #include "ec.cuh"
+#include "witness_program.hpp"
 #include <cstddef>
 #include <cstdint>
 
 namespace zke {
 namespace dev {
 
-static const int WITNESS_THREADS = 512;
+using zke::WITNESS_THREADS;   // witness_program.hpp: the stream's formats and constants
+using zke::WOP_NOP;
 static const uint32_t WITNESS_TERM_BUF = 8192;   // LC terms staged in shared memory per iteration (x 2 buffers x 8 B)
 
 // number of kernels launched by this library since load (reported by bench.py as gpu_launches)
@@ -22,24 +24,11 @@ inline int sm_count() {
     return n;
 }
 
-// Witness program resident in HBM (built once per circuit): a STREAM of fixed-size op records, one per thread and
-// iteration.  The levelised program of the front-end is cut into iterations of WITNESS_THREADS ops (levels are padded
-// with no-ops), so the kernel needs no level table and no LC pool indirection: iteration k, thread t executes
-// ops[k * WITNESS_THREADS + t]; the LC terms of an iteration's ops are one contiguous block of `terms`, described by
-// iter_hdr[k], which the CTA stages into shared memory one iteration ahead (cp.async) while it evaluates the current
-// one.  Everything that does not depend on witness data is therefore prefetched; the only dependent memory round
-// trip left in an iteration is the gather of the witness values themselves.
-//   op record  : x = dst, y = code | nA << 8 | nB << 13 | nC << 18, z = operand (first term index / source variable /
-//                aux offset), w = shift | nbits << 16 (OP_SHRAND)
-//   term       : {variable, coefficient index}; blocks of an op are laid out [A | B | C]
-static const uint32_t WOP_NOP = 15;
+// Witness program resident in HBM (built once per circuit): the stream of witness_program.hpp, which gives the formats.
 struct DevProgram {
     const uint4* ops;            // [n_iters][WITNESS_THREADS]
-    const uint4* iter_hdr;       // [n_iters + 2 * cluster]: {first term (even), term count (even), first cooperative op, their count
-                                 // | 1 << 31 on the iterations of a level's last round (cluster > 1: barrier across the CTAs)}
-    const uint32_t* coop;        // cooperative ops of the iterations (executed by the whole CTA), two words each:
-                                 // {offset into `aux`, 0}: native Sha256compression table ({n_desc, inputs[768],
-                                 // desc[n_desc][2]}, circuit.hpp: ShaBlock); {1 << 31 | offset into `aux`, dst}: FpMul hint
+    const uint4* iter_hdr;       // [n_iters + 2 * cluster]
+    const uint32_t* coop;        // cooperative ops of the iterations (executed by the whole CTA), two words each
     const uint2* terms;
     const uint32_t* aux;
     const uint8_t* coef_r;       // [n_coefs][32]: coefficient * R mod r  (Montgomery-scaled: (cR) (x) w = c*w)

@@ -19,6 +19,7 @@ cudaError_t upload_constants_verify(const FieldConsts*, const FieldConsts*);
 #include "../../include/zkemail_b200.h"
 #include "cuda_host.hpp"
 #include "engine.hpp"
+#include "witness_program.hpp"
 #include "binfile.hpp"
 #include "ec_host.hpp"
 #include "setup_host.hpp"
@@ -50,39 +51,6 @@ void zke::select_device(int device) {
 }
 
 namespace {
-
-// Fixed-operand form of a constant w (ff.cuh: Fp::mul_shoup): {w in standard form, floor(w 2^256 / r)}.  With
-// w 2^256 = q r + rem the remainder is the Montgomery image of w, so q = (w 2^256 - rem) / r exactly, and an exact
-// quotient is a product with r^-1 modulo 2^256: q = rem * (-r^-1 mod 2^256) mod 2^256 - no division.
-struct ShoupPair { U256 w, wq; };
-U256 mul_lo256(const U256& a, const U256& b) {
-    uint64_t t[4] = {0, 0, 0, 0};
-    for (int i = 0; i < 4; ++i) {
-        u128 c = 0;
-        for (int j = 0; i + j < 4; ++j) {
-            c += (u128)a.v[j] * b.v[i] + t[i + j];
-            t[i + j] = (uint64_t)c;
-            c >>= 64;
-        }
-    }
-    return U256{{t[0], t[1], t[2], t[3]}};
-}
-const U256& fr_neg_inv256() {     // -r^-1 mod 2^256 (Newton iteration from the 64-bit constant of the Montgomery product)
-    static const U256 v = [] {
-        const U256& p = fr_params().p;
-        U256 y = {{(uint64_t)0 - fr_params().inv, 0, 0, 0}};          // r^-1 mod 2^64
-        for (int it = 0; it < 2; ++it) {                               // y <- y (2 - r y): 64 -> 128 -> 256 bits
-            U256 t = mul_lo256(p, y), two = {{2, 0, 0, 0}}, d;
-            u256_sub(d, two, t);
-            y = mul_lo256(y, d);
-        }
-        U256 zero = {{0, 0, 0, 0}}, n;
-        u256_sub(n, zero, y);
-        return n;
-    }();
-    return v;
-}
-ShoupPair shoup_pair(const Fr& w) { return ShoupPair{w.to_u256(), mul_lo256(w.m, fr_neg_inv256())}; }
 
 // 32 x 256 window table of multiples of a generator, affine Montgomery, entry d = 0 is infinity
 template <class F>
@@ -583,6 +551,186 @@ static void check_key_matrices(const Circuit& c, const zke_zkey& zk) {
     compare("B", zk.b_ptr, zk.b_var, zk.b_coef, c.b_ptr, c.b_var, c.b_coef, false);
 }
 
+// Lowers the circuit's witness program into the kernel's stream (witness_program.cpp) with the options of this process and
+// context, and makes it resident.
+static void upload_program(zke_ctx* x, const Circuit& c) {
+    const uint32_t max_batch = x->max_batch;
+    LowerOptions opt;
+    // ZKE_NATIVE_SHA=0 keeps the Sha256compression gadget's own ops, ZKE_NATIVE_REGEX=0 turns the regex state seeding off,
+    // ZKE_COOP_FPMUL=0: the sequential single-thread hint
+    if (const char* e = getenv("ZKE_NATIVE_SHA")) opt.native_sha = atoi(e) != 0;
+    if (const char* e = getenv("ZKE_NATIVE_REGEX")) opt.native_regex = atoi(e) != 0;
+    if (const char* e = getenv("ZKE_COOP_FPMUL")) opt.coop_fpmul = atoi(e) != 0;
+    // ZKE_WITNESS_CLUSTER = 2 / 4 / 8: thread-block cluster of that many CTAs per email (witness.cu); every level is padded to
+    // whole rounds of `cluster` iterations, iteration k belongs to CTA k % cluster
+    // (default: as many CTAs per email as still fit one wave of the GPU's SMs at this context's batch size - a witness
+    // CTA owns an SM; ZKE_WITNESS_CLUSTER=1 keeps one CTA per email).
+    const uint32_t sms = (uint32_t)dev::sm_count();
+    opt.cluster = max_batch <= 8 ? 8 : (max_batch <= 32 ? 4 : (2 * max_batch <= sms ? 2 : 1));
+    if (const char* e = getenv("ZKE_WITNESS_CLUSTER")) { const int v = atoi(e); if (v == 1 || v == 2 || v == 4 || v == 8) opt.cluster = (uint32_t)v; }
+    WitnessStream S = lower_witness_program(c, x->coef_word, opt);
+    x->ops.upload(S.ops);
+    x->iter_hdr.upload(S.iter_hdr);
+    x->lc_terms.upload(S.terms);
+    x->aux.upload(S.aux);
+    x->coop.upload(S.coop);
+    x->iter_info = std::move(S.iter_info);
+    const uint32_t NSMALL = 4096;
+    std::vector<Fr> inv(NSMALL);
+    for (uint32_t i = 0; i < NSMALL; ++i) inv[i] = Fr::from_u64(i);
+    batch_inverse(inv.data(), NSMALL);
+    std::vector<U256> inv_std(NSMALL);
+    for (uint32_t i = 0; i < NSMALL; ++i) inv_std[i] = inv[i].to_u256();
+    x->small_inv.upload(inv_std);
+    dev::DevProgram& P = x->prog;
+    P.ops = (const uint4*)x->ops.p; P.iter_hdr = (const uint4*)x->iter_hdr.p; P.coop = (const uint32_t*)x->coop.p;
+    P.terms = (const uint2*)x->lc_terms.p; P.aux = (const uint32_t*)x->aux.p; P.coef_r = x->coef_r.p;
+    P.small_inv = x->small_inv.p; P.n_small_inv = NSMALL;
+    P.trace = nullptr;
+    P.cluster = S.cluster;
+    P.n_iters = S.n_iters; P.n_ops = (uint32_t)c.ops.size(); P.n_vars = c.n_vars; P.n_temps = c.n_temps;
+    P.n_outputs = c.n_outputs; P.n_inputs = c.n_inputs();
+}
+
+// R1CS (the circuit's A, B, C) or the QAP matrices of the key (A, B incl. the extra public rows; no C)
+static void upload_r1cs(zke_ctx* x, const Circuit* cp, const zke_zkey* zk) {
+    auto up_terms = [&](const std::vector<uint32_t>& var, const std::vector<uint32_t>& coef, DevBuf& dst) {
+        std::vector<uint32_t> t(2 * var.size() + 2);
+        for (size_t i = 0; i < var.size(); ++i) { t[2 * i] = var[i]; t[2 * i + 1] = x->coef_word[coef[i]]; }
+        dst.upload(t);
+    };
+    dev::DevR1cs& R = x->r1cs;
+    if (cp) {
+        const Circuit& c = *cp;
+        x->a_ptr.upload(c.a_ptr); x->b_ptr.upload(c.b_ptr); x->c_ptr.upload(c.c_ptr);
+        up_terms(c.a_var, c.a_coef, x->a_terms); up_terms(c.b_var, c.b_coef, x->b_terms); up_terms(c.c_var, c.c_coef, x->c_terms);
+        R.c_ptr = (const uint32_t*)x->c_ptr.p; R.c_terms = (const uint2*)x->c_terms.p;
+        R.n_constraints = c.n_constraints; R.n_public = c.n_public();
+    } else {
+        x->a_ptr.upload(zk->a_ptr); x->b_ptr.upload(zk->b_ptr);
+        up_terms(zk->a_var, zk->a_coef, x->a_terms); up_terms(zk->b_var, zk->b_coef, x->b_terms);
+        R.c_ptr = nullptr; R.c_terms = nullptr;
+        R.n_constraints = 1u << zk->log_n; R.n_public = 0;    // every domain row comes from the key's matrices
+    }
+    R.a_ptr = (const uint32_t*)x->a_ptr.p; R.b_ptr = (const uint32_t*)x->b_ptr.p;
+    R.a_terms = (const uint2*)x->a_terms.p; R.b_terms = (const uint2*)x->b_terms.p;
+    R.coef_r = x->coef_r.p; R.n_vars = x->n_vars;
+}
+
+namespace {
+// Fixed-operand form of a constant w (ff.cuh: Fp::mul_shoup): {w in standard form, floor(w 2^256 / r)}.  With
+// w 2^256 = q r + rem the remainder is the Montgomery image of w, so q = (w 2^256 - rem) / r exactly, and an exact
+// quotient is a product with r^-1 modulo 2^256: q = rem * (-r^-1 mod 2^256) mod 2^256 - no division.
+struct ShoupPair { U256 w, wq; };
+U256 mul_lo256(const U256& a, const U256& b) {
+    uint64_t t[4] = {0, 0, 0, 0};
+    for (int i = 0; i < 4; ++i) {
+        u128 c = 0;
+        for (int j = 0; i + j < 4; ++j) {
+            c += (u128)a.v[j] * b.v[i] + t[i + j];
+            t[i + j] = (uint64_t)c;
+            c >>= 64;
+        }
+    }
+    return U256{{t[0], t[1], t[2], t[3]}};
+}
+const U256& fr_neg_inv256() {     // -r^-1 mod 2^256 (Newton iteration from the 64-bit constant of the Montgomery product)
+    static const U256 v = [] {
+        const U256& p = fr_params().p;
+        U256 y = {{(uint64_t)0 - fr_params().inv, 0, 0, 0}};          // r^-1 mod 2^64
+        for (int it = 0; it < 2; ++it) {                               // y <- y (2 - r y): 64 -> 128 -> 256 bits
+            U256 t = mul_lo256(p, y), two = {{2, 0, 0, 0}}, d;
+            u256_sub(d, two, t);
+            y = mul_lo256(y, d);
+        }
+        U256 zero = {{0, 0, 0, 0}}, n;
+        u256_sub(n, zero, y);
+        return n;
+    }();
+    return v;
+}
+ShoupPair shoup_pair(const Fr& w) { return ShoupPair{w.to_u256(), mul_lo256(w.m, fr_neg_inv256())}; }
+}  // namespace
+
+static void build_ntt_tables(zke_ctx* x, unsigned log_n) {
+    const size_t N = (size_t)1 << log_n;
+    // twiddles omega^k, omega^-k (k < N/2) and the bit-reversed coset scale g^j / N
+    const Fr omega = fr_root_of_unity(log_n), omega_inv = omega.inv();
+    const Fr g = fr_root_of_unity(log_n + 1);
+    const Fr n_inv = Fr::from_u64(N).inv();
+    // constants of the transforms: Montgomery form (32 bytes) or fixed-operand pairs (64 bytes) - ZKE_NTT_SHOUP
+    bool shoup = false;
+    if (const char* e = getenv("ZKE_NTT_SHOUP")) shoup = atoi(e) != 0;
+    const size_t esz = shoup ? 64 : 32;
+    std::vector<uint8_t> fw(esz * std::max<size_t>(1, N / 2)), iv(esz * std::max<size_t>(1, N / 2)), cs(esz * N);
+    auto put = [&](std::vector<uint8_t>& tab, size_t i, const Fr& w) {
+        if (shoup) { const ShoupPair sp = shoup_pair(w); memcpy(&tab[64 * i], sp.w.v, 32); memcpy(&tab[64 * i + 32], sp.wq.v, 32); }
+        else memcpy(&tab[32 * i], w.m.v, 32);
+    };
+    const unsigned T = std::max(1u, std::min(16u, std::thread::hardware_concurrency()));
+    std::vector<std::thread> th;
+    for (unsigned t = 0; t < T; ++t) {
+        th.emplace_back([&, t]() {
+            size_t beg = (N / 2) * t / T, end = (N / 2) * (t + 1) / T;
+            if (beg < end) {
+                U256 e = {{(uint64_t)beg, 0, 0, 0}};
+                Fr a = omega.pow(e), b = omega_inv.pow(e);
+                for (size_t i = beg; i < end; ++i) { put(fw, i, a); put(iv, i, b); a = a * omega; b = b * omega_inv; }
+            }
+            beg = N * t / T; end = N * (t + 1) / T;
+            if (beg < end) {
+                U256 e = {{(uint64_t)beg, 0, 0, 0}};
+                Fr a = g.pow(e) * n_inv;
+                for (size_t j = beg; j < end; ++j) {
+                    size_t p = 0;
+                    for (unsigned bit = 0; bit < log_n; ++bit) if (j & ((size_t)1 << bit)) p |= (size_t)1 << (log_n - 1 - bit);
+                    put(cs, p, a);
+                    a = a * g;
+                }
+            }
+        });
+    }
+    for (auto& t : th) t.join();
+    if (N == 1) { put(fw, 0, Fr::one()); put(iv, 0, Fr::one()); }
+    x->tw_fwd.upload(fw); x->tw_inv.upload(iv); x->coset_scale.upload(cs);
+    x->ntt.tw_fwd = x->tw_fwd.p; x->ntt.tw_inv = x->tw_inv.p; x->ntt.log_n = (int)log_n; x->ntt.shoup = shoup;
+}
+
+// The proving lanes of a context with a key: streams, NTT vectors and MSM workspace each.
+static void open_lanes(zke_ctx* x, size_t N, int prio_least, int prio_greatest) {
+    const uint32_t max_batch = x->max_batch;
+    x->cfg_w = dev::msm_config_witness();
+    x->cfg_h = x->zkey->cfg_h;
+    size_t ws = std::max(dev::MsmPlan<dev::Fq>::workspace_bytes(x->n_vars, x->cfg_w),
+                         dev::MsmPlan<dev::Fq>::workspace_bytes((uint32_t)N, x->cfg_h));
+    ws = std::max(ws, dev::MsmPlan<dev::Fq2>::workspace_bytes(x->n_vars, x->cfg_w));
+    int want = 8;
+    if (const char* e = getenv("ZKE_LANES")) want = atoi(e);
+    if (const char* e = getenv("ZKE_SPLIT_STREAMS")) x->split_streams = atoi(e) != 0;
+    if (const char* e = getenv("ZKE_FINISH_THREADS")) x->finish_threads = std::max(1, std::min(32, atoi(e)));
+    want = std::max(1, std::min(ZKE_MAX_LANES, std::min<int>(want, (int)max_batch)));
+    {   // lanes only buy overlap: open no more than fit in device memory beside the second witness slot (allocated by
+        // the first zke_fullprove_submit) and 1 GiB for per-call buffers - at 2^24 eight lanes alone exceed 80 GB
+        size_t free_b = 0, total_b = 0;
+        CUDA_OK(cudaMemGetInfo(&free_b, &total_b));
+        const size_t lane_bytes = 4 * N * 32 + ws;
+        const size_t keep = x->stride * 32 * max_batch + ((size_t)1 << 30);
+        const size_t fit = free_b > keep ? (free_b - keep) / lane_bytes : 0;
+        want = std::max(1, std::min<int>(want, (int)std::min<size_t>(fit, ZKE_MAX_LANES)));
+    }
+    // the lanes' light streams sit one priority step below the witness stream (when the device offers three levels)
+    const int prio_light = prio_greatest < prio_least - 1 ? prio_greatest + 1 : prio_greatest;
+    for (int i = 0; i < want; ++i) {
+        zke_ctx::Lane& L = x->lanes[i];
+        CUDA_OK(cudaStreamCreateWithPriority(&L.st, cudaStreamNonBlocking, prio_light));
+        CUDA_OK(cudaStreamCreateWithPriority(&L.heavy, cudaStreamNonBlocking, prio_least));
+        for (auto& e : L.ev) CUDA_OK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+        L.va.alloc(N * 32); L.vb.alloc(N * 32); L.vc.alloc(N * 32); L.vd.alloc(N * 32);
+        L.msm_ws.alloc(ws);
+    }
+    x->lanes_alloc = x->n_lanes = want;
+}
+
 static zke_ctx* do_open(const zke_circuit* zc, const zke_zkey* zk, int device, uint32_t max_batch) {
     select_device(device);
     const Circuit* cp = zc ? &zc->c : nullptr;
@@ -602,27 +750,8 @@ static zke_ctx* do_open(const zke_circuit* zc, const zke_zkey* zk, int device, u
 
     // coefficient words (lc_term.cuh) of the circuit's - or the key's - interned coefficient table
     const std::vector<U256>& coefs = cp ? cp->coefs : zk->coefs;
-    {
-        std::vector<uint32_t>& coef_word = x->coef_word;
-        coef_word.assign(coefs.size(), 0);
-        if (coefs.size() >= (1u << 24)) throw std::runtime_error("too many distinct coefficients");
-        for (size_t i = 0; i < coefs.size(); ++i) {
-            auto log2_exact = [](const U256& v) -> int {   // k if v == 2^k, else -1
-                int k = -1, bits = 0;
-                for (unsigned b = 0; b < 256; ++b) if (u256_bit(v, b)) { k = (int)b; ++bits; }
-                return bits == 1 ? k : -1;
-            };
-            U256 neg;
-            u256_sub(neg, fr_params().p, coefs[i]);
-            const int kp = log2_exact(coefs[i]), kn = log2_exact(neg);
-            uint32_t kind = 4, k = 0;
-            if (kp == 0) kind = 0;
-            else if (kn == 0) kind = 1;
-            else if (kp > 0 && kp <= 252 && i <= 0xffffu) { kind = 2; k = (uint32_t)kp; }
-            else if (kn > 0 && kn <= 252 && i <= 0xffffu) { kind = 3; k = (uint32_t)kn; }
-            coef_word[i] = kind == 4 ? ((uint32_t)i | (4u << 24)) : (((uint32_t)i & 0xffffu) | (k << 16) | (kind << 24));
-        }
-        // coefficient table scaled by R: as Montgomery numbers these are just the Montgomery forms
+    x->coef_word = coef_words(coefs);
+    {   // coefficient table scaled by R: as Montgomery numbers these are just the Montgomery forms
         std::vector<Fr> cr(std::max<size_t>(1, coefs.size()));
         for (size_t i = 0; i < coefs.size(); ++i) cr[i] = Fr::from_u256(coefs[i]);
         x->coef_r.upload(cr);
@@ -632,305 +761,8 @@ static zke_ctx* do_open(const zke_circuit* zc, const zke_zkey* zk, int device, u
     if (zk && cp && cp->r1cs_only && zk->has_coefs) check_key_matrices(*cp, *zk);
 
     // witness program (none for a circuit read from an `.r1cs`: its witnesses are loaded)
-    if (cp && !cp->r1cs_only) {
-        const Circuit& c = *cp;
-        // Streamed witness program (device_engine.cuh): per level, ops sorted by kind / size so that the threads of an
-        // iteration do similar work, padded with no-ops to whole iterations of WITNESS_THREADS records; the LC terms
-        // of an iteration form one contiguous, 16-byte aligned block.
-        const uint32_t T = dev::WITNESS_THREADS;
-        std::vector<uint32_t> packed;                 // 4 words per record
-        std::vector<uint32_t> terms, hdr;             // 2 words per term / per iteration header
-        packed.reserve(4 * (c.ops.size() + (size_t)T * c.n_levels()));
-        terms.reserve(2 * c.lc_var.size() + 16);
-        auto lc_len = [&](uint32_t id) { return c.lc_ptr[id + 1] - c.lc_ptr[id]; };
-        const std::vector<uint32_t>& coef_word = x->coef_word;
-        // the device's big-integer hint works on at most 20 limbs (witness.cu: fpmul_hint_dev); refuse larger FpMul
-        // instances here instead of producing a witness that fails its constraints later
-        for (const WOp& o : c.ops)
-            if (o.code == OP_FPMUL && c.aux[o.a + 1] > 20) throw std::runtime_error("FpMul with k = " + std::to_string(c.aux[o.a + 1]) + " limbs exceeds the device hint's limit of 20");
-        // ---- native Sha256compression (circuit.hpp: ShaBlock; ZKE_NATIVE_SHA=0 keeps the gadget's own ops): the ops that
-        // define the signals / scratch slots of a recorded instance are replaced by ONE cooperative op per instance and
-        // the program is levelised again - the chained compressions then cost one level each instead of ~320.
-        bool native_sha = !c.sha_blocks.empty();
-        if (const char* e = getenv("ZKE_NATIVE_SHA")) native_sha = native_sha && atoi(e) != 0;
-        // ---- zk-regex state seeding (circuit.hpp: RegexSeed; ZKE_NATIVE_REGEX=0 turns it off): one cooperative op per regex
-        // instance runs the automaton over the message and writes every state signal; the instance's own ops stay (they
-        // write the same values again) but now depend on seeded signals instead of on the previous position's gadgets, so the
-        // ~4 levels per message byte collapse into a handful for the whole message.
-        bool native_rx = !c.regex_seeds.empty();
-        if (const char* e = getenv("ZKE_NATIVE_REGEX")) native_rx = native_rx && atoi(e) != 0;
-        static const uint32_t XOP_SHA = 6, XOP_RX = 7;
-        std::vector<WOp> xops;                         // code XOP_SHA: a = index of the block; XOP_RX: a = index of the seed
-        std::vector<uint32_t> xlevel_ptr;              // ops of level l: [xlevel_ptr[l], xlevel_ptr[l + 1])
-        std::vector<uint32_t> aux = c.aux;
-        std::vector<uint32_t> sha_aux_off(c.sha_blocks.size(), 0), rx_aux_off(c.regex_seeds.size(), 0);
-        if (!native_sha && !native_rx) {
-            xops = c.ops;
-            xlevel_ptr = c.level_ptr;
-        } else {
-            const uint32_t total = c.n_vars + c.n_temps;
-            std::vector<int32_t> owner(total, -1);     // slot -> block that defines it
-            std::vector<uint8_t> seeded(total, 0);     // slot written by a regex seed op (its own op stays)
-            if (native_rx)
-                for (size_t ri = 0; ri < c.regex_seeds.size(); ++ri) {
-                    const RegexSeed& R = c.regex_seeds[ri];
-                    rx_aux_off[ri] = (uint32_t)aux.size();
-                    append_regex_seed(aux, R);
-                    for (size_t d = 0; d < R.desc.size(); d += 2) seeded[R.desc[d]] = 1;
-                }
-            if (aux.size() >= (1u << 30)) throw std::runtime_error("witness program: auxiliary table too large");
-            for (size_t bi = 0; native_sha && bi < c.sha_blocks.size(); ++bi) {
-                const ShaBlock& B = c.sha_blocks[bi];
-                for (uint32_t v = B.var_begin; v < B.var_end; ++v) owner[v] = (int32_t)bi;
-                for (uint32_t v = B.temp_begin; v < B.temp_end; ++v) owner[v] = (int32_t)bi;
-                sha_aux_off[bi] = (uint32_t)aux.size();
-                aux.push_back((uint32_t)(B.desc.size() / 2));
-                aux.insert(aux.end(), B.inputs.begin(), B.inputs.end());
-                aux.insert(aux.end(), B.desc.begin(), B.desc.end());
-            }
-            // Order: c.ops is in level order (producers before consumers).  A block's op is inserted right after the
-            // producer of its LAST-defined input: everything it reads precedes it, and everything that reads its outputs
-            // (the final-sum bits, originally defined after all of the block's inputs) follows it.
-            std::vector<int64_t> def_pos(total, -1);
-            for (size_t i = 0; i < c.ops.size(); ++i) {
-                const WOp& o = c.ops[i];
-                const uint32_t nd = o.code == OP_FPMUL ? 2 * c.aux[o.a + 1] : 1;
-                for (uint32_t j = 0; j < nd; ++j) def_pos[o.dst + j] = (int64_t)i;
-            }
-            std::vector<std::vector<uint32_t>> blocks_at(c.ops.size() + 1), seeds_at(c.ops.size() + 1);
-            for (size_t bi = 0; native_sha && bi < c.sha_blocks.size(); ++bi) {
-                int64_t pos = 0;
-                for (uint32_t v : c.sha_blocks[bi].inputs) if (v < SHA_CONST0) pos = std::max(pos, def_pos[v] + 1);
-                blocks_at[(size_t)pos].push_back((uint32_t)bi);
-            }
-            for (size_t ri = 0; native_rx && ri < c.regex_seeds.size(); ++ri) {
-                int64_t pos = 0;      // right after the producer of the last message byte: before every op of the instance
-                for (uint32_t v : c.regex_seeds[ri].bytes) pos = std::max(pos, def_pos[v] + 1);
-                seeds_at[(size_t)pos].push_back((uint32_t)ri);
-            }
-            std::vector<WOp> kept;
-            kept.reserve(c.ops.size());
-            for (size_t i = 0; i <= c.ops.size(); ++i) {
-                for (uint32_t bi : blocks_at[i]) kept.push_back(WOp{XOP_SHA, c.sha_blocks[bi].var_begin, bi, 0, 0});
-                for (uint32_t ri : seeds_at[i]) kept.push_back(WOp{XOP_RX, 0, ri, 0, 0});
-                if (i < c.ops.size() && owner[c.ops[i].dst] < 0) kept.push_back(c.ops[i]);
-            }
-            // levelise (the same rules as Builder::finalize, plus the multi-output block op)
-            std::vector<uint32_t> level(total, 0), op_level(kept.size(), 0);
-            std::vector<uint8_t> defined(total, 0);
-            defined[0] = 1;
-            for (auto& g : c.groups) if (g.kind != 0) for (uint32_t i = 0; i < g.count; ++i) defined[g.first + i] = 1;
-            auto need = [&](uint32_t v) -> uint32_t {
-                if (!defined[v]) throw std::runtime_error("native SHA substitution: an op reads an unassigned signal");
-                return level[v];
-            };
-            auto lc_level = [&](uint32_t id) { uint32_t l = 0; for (uint32_t k = c.lc_ptr[id]; k < c.lc_ptr[id + 1]; ++k) l = std::max(l, need(c.lc_var[k])); return l; };
-            uint32_t max_level = 0;
-            for (size_t i = 0; i < kept.size(); ++i) {
-                const WOp& o = kept[i];
-                uint32_t l = 0;
-                switch (o.code) {
-                    case OP_LIN: case OP_SHRLC: l = lc_level(o.a); break;
-                    case OP_QUAD: l = std::max(lc_level(o.a), std::max(lc_level(o.b), lc_level(o.c))); break;
-                    case OP_SHRAND: case OP_INVZ: l = need(o.a); break;
-                    case OP_FPMUL: { const uint32_t kk = c.aux[o.a + 1]; for (uint32_t j = 0; j < 3 * kk; ++j) l = std::max(l, need(c.aux[o.a + 2 + j])); break; }
-                    case XOP_SHA: for (uint32_t v : c.sha_blocks[o.a].inputs) if (v < SHA_CONST0) l = std::max(l, need(v)); break;
-                    case XOP_RX: for (uint32_t v : c.regex_seeds[o.a].bytes) l = std::max(l, need(v)); break;
-                    default: throw std::runtime_error("bad opcode");
-                }
-                l += 1;
-                if (o.code == XOP_SHA) {
-                    const ShaBlock& B = c.sha_blocks[o.a];
-                    for (uint32_t v = B.var_begin; v < B.var_end; ++v) { defined[v] = 1; level[v] = l; }
-                } else if (o.code == XOP_RX) {
-                    const RegexSeed& R = c.regex_seeds[o.a];
-                    for (size_t d = 0; d < R.desc.size(); d += 2) { defined[R.desc[d]] = 1; level[R.desc[d]] = l; }
-                } else if (o.code == OP_FPMUL) {
-                    const uint32_t kk = c.aux[o.a + 1];
-                    for (uint32_t j = 0; j < 2 * kk; ++j) { defined[o.dst + j] = 1; level[o.dst + j] = l; }
-                } else if (seeded[o.dst]) {
-                    // the value is already there (same value, written by the seed op at an earlier level): readers keep
-                    // depending on the seed, this op only has to run after its own operands
-                    if (!defined[o.dst]) throw std::runtime_error("regex seeding: a seeded signal is produced before its seed op");
-                } else {
-                    defined[o.dst] = 1; level[o.dst] = l;
-                }
-                op_level[i] = l;
-                max_level = std::max(max_level, l);
-            }
-            xlevel_ptr.assign(max_level + 1, 0);
-            for (uint32_t l : op_level) xlevel_ptr[l]++;                 // levels are 1-based here
-            { uint32_t run = 0; for (uint32_t l = 1; l <= max_level; ++l) { const uint32_t n = xlevel_ptr[l]; xlevel_ptr[l] = run; run += n; } xlevel_ptr[0] = 0; }
-            xops.resize(kept.size());
-            { std::vector<uint32_t> cursor(xlevel_ptr.begin(), xlevel_ptr.end()); for (size_t i = 0; i < kept.size(); ++i) xops[cursor[op_level[i]]++] = kept[i]; }
-            std::vector<uint32_t> lp(max_level + 1);
-            for (uint32_t l = 1; l <= max_level; ++l) lp[l - 1] = xlevel_ptr[l];
-            lp[max_level] = (uint32_t)kept.size();
-            xlevel_ptr.swap(lp);
-        }
-        const uint32_t n_xlevels = xlevel_ptr.empty() ? 0 : (uint32_t)xlevel_ptr.size() - 1;
-        std::vector<uint32_t> coop;                     // cooperative ops (two words each), grouped by iteration
-        bool coop_fpmul = true;                         // ZKE_COOP_FPMUL=0: the sequential single-thread hint
-        if (const char* e = getenv("ZKE_COOP_FPMUL")) coop_fpmul = atoi(e) != 0;
-        std::vector<uint32_t> order;
-        std::vector<uint64_t> keys;
-        // ZKE_WITNESS_CLUSTER = 2 / 4 / 8: thread-block cluster of that many CTAs per email (witness.cu); every level is padded to
-        // whole rounds of `cluster` iterations, iteration k belongs to CTA k % cluster
-        // (default: as many CTAs per email as still fit one wave of the GPU's SMs at this context's batch size - a witness
-        // CTA owns an SM; ZKE_WITNESS_CLUSTER=1 keeps one CTA per email).
-        const uint32_t sms = (uint32_t)dev::sm_count();
-        uint32_t cluster = max_batch <= 8 ? 8 : (max_batch <= 32 ? 4 : (2 * max_batch <= sms ? 2 : 1));
-        if (const char* e = getenv("ZKE_WITNESS_CLUSTER")) { const int v = atoi(e); if (v == 1 || v == 2 || v == 4 || v == 8) cluster = (uint32_t)v; }
-        std::vector<std::pair<size_t, size_t>> level_iters;   // per level: index of its first iteration, number of non-empty ones
-        for (uint32_t lvl = 0; lvl < n_xlevels; ++lvl) {
-            const uint32_t beg = xlevel_ptr[lvl], end = xlevel_ptr[lvl + 1];
-            const size_t level_first_iter = hdr.size() / 4;
-            order.clear();
-            const uint32_t coop_first = (uint32_t)(coop.size() / 2);
-            for (uint32_t i = beg; i < end; ++i) {
-                if (xops[i].code == XOP_SHA) { coop.push_back(sha_aux_off[xops[i].a]); coop.push_back(0); }
-                else if (xops[i].code == XOP_RX) { coop.push_back(0x40000000u | rx_aux_off[xops[i].a]); coop.push_back(0); }
-                else if (xops[i].code == OP_FPMUL && coop_fpmul) { coop.push_back(0x80000000u | xops[i].a); coop.push_back(xops[i].dst); }
-                else order.push_back(i);
-            }
-            uint32_t coop_left = (uint32_t)(coop.size() / 2) - coop_first;   // attached to the level's first iteration
-            // Sort key: kind, then the positions of the terms that need a product (coefficient other than +-1) in the
-            // flattened [A | B | C] term list, then the term count.  Within an LC the product terms are emitted first
-            // (addition commutes), so the ops of a warp take the product branch of eval_lcs in the same term slots -
-            // or not at all: a warp only pays for a Montgomery product where some lane needs one.
-            auto key = [&](uint32_t i) -> uint64_t {
-                const WOp& o = xops[i];
-                if (o.code == OP_FPMUL) return ~0ull;
-                if (o.code == OP_INVZ) return 1ull << 62;
-                if (o.code == OP_SHRAND) return 0;
-                const uint32_t ids[3] = {o.a, o.b, o.c};
-                const uint32_t n_lc = o.code == OP_QUAD ? 3 : 1;
-                uint64_t mask = 0;
-                uint32_t pos = 0;
-                for (uint32_t q = 0; q < n_lc; ++q) {
-                    uint32_t heavy = 0;
-                    for (uint32_t k = c.lc_ptr[ids[q]]; k < c.lc_ptr[ids[q] + 1]; ++k) heavy += (coef_word[c.lc_coef[k]] >> 24) >= 2;
-                    for (uint32_t t = 0; t < heavy && pos + t < 48; ++t) mask |= 1ull << (pos + t);
-                    pos += lc_len(ids[q]);
-                }
-                return ((uint64_t)(o.code == OP_QUAD ? 2 : 1) << 60) | (mask << 8) | std::min<uint32_t>(pos, 255);
-            };
-            std::vector<std::pair<uint64_t, uint32_t>> keyed(order.size());
-            for (size_t i = 0; i < order.size(); ++i) keyed[i] = {key(order[i]), order[i]};
-            std::stable_sort(keyed.begin(), keyed.end(), [](const std::pair<uint64_t, uint32_t>& x, const std::pair<uint64_t, uint32_t>& y) { return x.first > y.first; });
-            for (size_t i = 0; i < order.size(); ++i) order[i] = keyed[i].second;
-            const size_t n_regular = order.size();
-            for (size_t base = 0; base < std::max<size_t>(n_regular, coop_left ? 1 : 0); base += T) {
-                const uint32_t first_term = (uint32_t)(terms.size() / 2);
-                for (uint32_t t = 0; t < T; ++t) {
-                    uint32_t rec[4] = {0, dev::WOP_NOP, 0, 0};
-                    if (base + t < n_regular) {
-                        const WOp& o = xops[order[base + t]];
-                        rec[0] = o.dst;
-                        if (o.code == OP_LIN || o.code == OP_QUAD || o.code == OP_SHRLC) {
-                            const uint32_t ids[3] = {o.a, o.b, o.c};
-                            const uint32_t n_lc = o.code == OP_QUAD ? 3 : 1;
-                            uint32_t n[3] = {0, 0, 0};
-                            rec[2] = (uint32_t)(terms.size() / 2);
-                            for (uint32_t q = 0; q < n_lc; ++q) {
-                                n[q] = lc_len(ids[q]);
-                                if (n[q] > 31) throw std::runtime_error("linear combination too long for the streamed witness program");
-                                for (int pass = 0; pass < 2; ++pass)   // product terms first
-                                    for (uint32_t k = c.lc_ptr[ids[q]]; k < c.lc_ptr[ids[q] + 1]; ++k)
-                                        if (((coef_word[c.lc_coef[k]] >> 24) >= 2) == (pass == 0)) { terms.push_back(c.lc_var[k]); terms.push_back(coef_word[c.lc_coef[k]]); }
-                            }
-                            rec[1] = o.code | (n[0] << 8) | (n[1] << 13) | (n[2] << 18);
-                            if (o.code == OP_SHRLC) {
-                                if (o.b > 0xffffu || o.c > 0xffffu) throw std::runtime_error("OP_SHRLC operand out of range");
-                                rec[3] = o.b | (o.c << 16);
-                            }
-                        } else if (o.code == OP_SHRAND) {
-                            if (o.b > 0xffffu || o.c > 0xffffu) throw std::runtime_error("OP_SHRAND operand out of range");
-                            rec[1] = o.code; rec[2] = o.a; rec[3] = o.b | (o.c << 16);
-                        } else {
-                            rec[1] = o.code; rec[2] = o.a;
-                        }
-                    }
-                    packed.insert(packed.end(), rec, rec + 4);
-                }
-                if ((terms.size() / 2) & 1) { terms.push_back(0); terms.push_back(0); }   // keep blocks 16-byte aligned
-                hdr.push_back(first_term);
-                hdr.push_back((uint32_t)(terms.size() / 2) - first_term);
-                hdr.push_back(coop_first);
-                hdr.push_back(coop_left);
-                coop_left = 0;
-                x->iter_info.push_back(packed[packed.size() - 4 * T + 1]);
-                x->iter_info.push_back((uint32_t)std::min<size_t>(T, n_regular > base ? n_regular - base : 0));
-                x->iter_info.push_back((uint32_t)(terms.size() / 2) - first_term);
-            }
-            // pad the level to whole rounds (empty iterations: no-op records, no terms)
-            level_iters.emplace_back(level_first_iter, hdr.size() / 4 - level_first_iter);
-            while (cluster > 1 && (hdr.size() / 4 - level_first_iter) % cluster != 0) {
-                for (uint32_t t = 0; t < T; ++t) { const uint32_t rec[4] = {0, dev::WOP_NOP, 0, 0}; packed.insert(packed.end(), rec, rec + 4); }
-                hdr.push_back((uint32_t)(terms.size() / 2)); hdr.push_back(0); hdr.push_back((uint32_t)(coop.size() / 2)); hdr.push_back(0);
-                x->iter_info.push_back(dev::WOP_NOP); x->iter_info.push_back(0); x->iter_info.push_back(0);
-            }
-        }
-        const uint32_t n_iters = (uint32_t)(hdr.size() / 4);
-        // Cluster barrier flags (bit 31 of header word 3, on every iteration of a level's last round): needed when signals cross
-        // CTAs - the level had more than one iteration (other CTAs wrote) or the next one has (other CTAs will read).  Runs of
-        // one-iteration levels (the Poseidon rounds, the tails of the comparison chains) stay on CTA 0 with its own barrier.
-        for (size_t l = 0; l < level_iters.size(); ++l) {
-            const bool last = l + 1 == level_iters.size();
-            if (!(level_iters[l].second > 1 || last || level_iters[l + 1].second > 1)) continue;
-            const size_t end_iter = last ? n_iters : level_iters[l + 1].first;
-            for (uint32_t q = 1; q <= cluster && end_iter >= level_iters[l].first + q; ++q) hdr[4 * (end_iter - q) + 3] |= 0x80000000u;
-        }
-        for (uint32_t q = 0; q < 2 * cluster; ++q) { hdr.push_back((uint32_t)(terms.size() / 2)); hdr.push_back(0); hdr.push_back(0); hdr.push_back(0); }   // sentinel headers
-        if (packed.empty()) packed.resize(4 * T, 0);
-        for (int q = 0; q < 8; ++q) terms.push_back(0);
-        x->ops.upload(packed);
-        x->iter_hdr.upload(hdr);
-        x->lc_terms.upload(terms);
-        if (aux.empty()) aux.push_back(0);
-        x->aux.upload(aux);
-        if (coop.empty()) { coop.push_back(0); coop.push_back(0); }
-        x->coop.upload(coop);
-        const uint32_t NSMALL = 4096;
-        std::vector<Fr> inv(NSMALL);
-        for (uint32_t i = 0; i < NSMALL; ++i) inv[i] = Fr::from_u64(i);
-        batch_inverse(inv.data(), NSMALL);
-        std::vector<U256> inv_std(NSMALL);
-        for (uint32_t i = 0; i < NSMALL; ++i) inv_std[i] = inv[i].to_u256();
-        x->small_inv.upload(inv_std);
-        dev::DevProgram& P = x->prog;
-        P.ops = (const uint4*)x->ops.p; P.iter_hdr = (const uint4*)x->iter_hdr.p; P.coop = (const uint32_t*)x->coop.p;
-        P.terms = (const uint2*)x->lc_terms.p; P.aux = (const uint32_t*)x->aux.p; P.coef_r = x->coef_r.p;
-        P.small_inv = x->small_inv.p; P.n_small_inv = NSMALL;
-        P.trace = nullptr;
-        P.cluster = cluster;
-        P.n_iters = n_iters; P.n_ops = (uint32_t)c.ops.size(); P.n_vars = c.n_vars; P.n_temps = c.n_temps;
-        P.n_outputs = c.n_outputs; P.n_inputs = c.n_inputs();
-    }
-    // R1CS (the circuit's A, B, C) or the QAP matrices of the key (A, B incl. the extra public rows; no C)
-    {
-        auto up_terms = [&](const std::vector<uint32_t>& var, const std::vector<uint32_t>& coef, DevBuf& dst) {
-            std::vector<uint32_t> t(2 * var.size() + 2);
-            for (size_t i = 0; i < var.size(); ++i) { t[2 * i] = var[i]; t[2 * i + 1] = x->coef_word[coef[i]]; }
-            dst.upload(t);
-        };
-        dev::DevR1cs& R = x->r1cs;
-        if (cp) {
-            const Circuit& c = *cp;
-            x->a_ptr.upload(c.a_ptr); x->b_ptr.upload(c.b_ptr); x->c_ptr.upload(c.c_ptr);
-            up_terms(c.a_var, c.a_coef, x->a_terms); up_terms(c.b_var, c.b_coef, x->b_terms); up_terms(c.c_var, c.c_coef, x->c_terms);
-            R.c_ptr = (const uint32_t*)x->c_ptr.p; R.c_terms = (const uint2*)x->c_terms.p;
-            R.n_constraints = c.n_constraints; R.n_public = c.n_public();
-        } else {
-            x->a_ptr.upload(zk->a_ptr); x->b_ptr.upload(zk->b_ptr);
-            up_terms(zk->a_var, zk->a_coef, x->a_terms); up_terms(zk->b_var, zk->b_coef, x->b_terms);
-            R.c_ptr = nullptr; R.c_terms = nullptr;
-            R.n_constraints = 1u << zk->log_n; R.n_public = 0;    // every domain row comes from the key's matrices
-        }
-        R.a_ptr = (const uint32_t*)x->a_ptr.p; R.b_ptr = (const uint32_t*)x->b_ptr.p;
-        R.a_terms = (const uint2*)x->a_terms.p; R.b_terms = (const uint2*)x->b_terms.p;
-        R.coef_r = x->coef_r.p; R.n_vars = x->n_vars;
-    }
+    if (cp && !cp->r1cs_only) upload_program(x.get(), *cp);
+    upload_r1cs(x.get(), cp, zk);
     x->stride = (size_t)x->n_vars + (cp ? cp->n_temps : 0);
     x->inputs.alloc((size_t)std::max(1u, x->n_inputs) * 32 * max_batch);
     x->check_flag.alloc(8);
@@ -938,78 +770,8 @@ static zke_ctx* do_open(const zke_circuit* zc, const zke_zkey* zk, int device, u
     alloc_slot(x.get(), x->slots[0]);
 
     if (zk) {
-        const unsigned log_n = zk->log_n;
-        const size_t N = (size_t)1 << log_n;
-        // twiddles omega^k, omega^-k (k < N/2) and the bit-reversed coset scale g^j / N
-        const Fr omega = fr_root_of_unity(log_n), omega_inv = omega.inv();
-        const Fr g = fr_root_of_unity(log_n + 1);
-        const Fr n_inv = Fr::from_u64(N).inv();
-        // constants of the transforms: Montgomery form (32 bytes) or fixed-operand pairs (64 bytes) - ZKE_NTT_SHOUP
-        bool shoup = false;
-        if (const char* e = getenv("ZKE_NTT_SHOUP")) shoup = atoi(e) != 0;
-        const size_t esz = shoup ? 64 : 32;
-        std::vector<uint8_t> fw(esz * std::max<size_t>(1, N / 2)), iv(esz * std::max<size_t>(1, N / 2)), cs(esz * N);
-        auto put = [&](std::vector<uint8_t>& tab, size_t i, const Fr& w) {
-            if (shoup) { const ShoupPair sp = shoup_pair(w); memcpy(&tab[64 * i], sp.w.v, 32); memcpy(&tab[64 * i + 32], sp.wq.v, 32); }
-            else memcpy(&tab[32 * i], w.m.v, 32);
-        };
-        const unsigned T = std::max(1u, std::min(16u, std::thread::hardware_concurrency()));
-        std::vector<std::thread> th;
-        for (unsigned t = 0; t < T; ++t) {
-            th.emplace_back([&, t]() {
-                size_t beg = (N / 2) * t / T, end = (N / 2) * (t + 1) / T;
-                if (beg < end) {
-                    U256 e = {{(uint64_t)beg, 0, 0, 0}};
-                    Fr a = omega.pow(e), b = omega_inv.pow(e);
-                    for (size_t i = beg; i < end; ++i) { put(fw, i, a); put(iv, i, b); a = a * omega; b = b * omega_inv; }
-                }
-                beg = N * t / T; end = N * (t + 1) / T;
-                if (beg < end) {
-                    U256 e = {{(uint64_t)beg, 0, 0, 0}};
-                    Fr a = g.pow(e) * n_inv;
-                    for (size_t j = beg; j < end; ++j) {
-                        size_t p = 0;
-                        for (unsigned bit = 0; bit < log_n; ++bit) if (j & ((size_t)1 << bit)) p |= (size_t)1 << (log_n - 1 - bit);
-                        put(cs, p, a);
-                        a = a * g;
-                    }
-                }
-            });
-        }
-        for (auto& t : th) t.join();
-        if (N == 1) { put(fw, 0, Fr::one()); put(iv, 0, Fr::one()); }
-        x->tw_fwd.upload(fw); x->tw_inv.upload(iv); x->coset_scale.upload(cs);
-        x->ntt.tw_fwd = x->tw_fwd.p; x->ntt.tw_inv = x->tw_inv.p; x->ntt.log_n = (int)log_n; x->ntt.shoup = shoup;
-        x->cfg_w = dev::msm_config_witness();
-        x->cfg_h = zk->cfg_h;
-        size_t ws = std::max(dev::MsmPlan<dev::Fq>::workspace_bytes(x->n_vars, x->cfg_w),
-                             dev::MsmPlan<dev::Fq>::workspace_bytes((uint32_t)N, x->cfg_h));
-        ws = std::max(ws, dev::MsmPlan<dev::Fq2>::workspace_bytes(x->n_vars, x->cfg_w));
-        int want = 8;
-        if (const char* e = getenv("ZKE_LANES")) want = atoi(e);
-        if (const char* e = getenv("ZKE_SPLIT_STREAMS")) x->split_streams = atoi(e) != 0;
-        if (const char* e = getenv("ZKE_FINISH_THREADS")) x->finish_threads = std::max(1, std::min(32, atoi(e)));
-        want = std::max(1, std::min(ZKE_MAX_LANES, std::min<int>(want, (int)max_batch)));
-        {   // lanes only buy overlap: open no more than fit in device memory beside the second witness slot (allocated by
-            // the first zke_fullprove_submit) and 1 GiB for per-call buffers - at 2^24 eight lanes alone exceed 80 GB
-            size_t free_b = 0, total_b = 0;
-            CUDA_OK(cudaMemGetInfo(&free_b, &total_b));
-            const size_t lane_bytes = 4 * N * 32 + ws;
-            const size_t keep = x->stride * 32 * max_batch + ((size_t)1 << 30);
-            const size_t fit = free_b > keep ? (free_b - keep) / lane_bytes : 0;
-            want = std::max(1, std::min<int>(want, (int)std::min<size_t>(fit, ZKE_MAX_LANES)));
-        }
-        // the lanes' light streams sit one priority step below the witness stream (when the device offers three levels)
-        const int prio_light = prio_greatest < prio_least - 1 ? prio_greatest + 1 : prio_greatest;
-        for (int i = 0; i < want; ++i) {
-            zke_ctx::Lane& L = x->lanes[i];
-            CUDA_OK(cudaStreamCreateWithPriority(&L.st, cudaStreamNonBlocking, prio_light));
-            CUDA_OK(cudaStreamCreateWithPriority(&L.heavy, cudaStreamNonBlocking, prio_least));
-            for (auto& e : L.ev) CUDA_OK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-            L.va.alloc(N * 32); L.vb.alloc(N * 32); L.vc.alloc(N * 32); L.vd.alloc(N * 32);
-            L.msm_ws.alloc(ws);
-        }
-        x->lanes_alloc = x->n_lanes = want;
+        build_ntt_tables(x.get(), zk->log_n);
+        open_lanes(x.get(), (size_t)1 << zk->log_n, prio_least, prio_greatest);
     }
     CUDA_OK(cudaDeviceSynchronize());
     return x.release();

@@ -1,5 +1,5 @@
 // Evaluation of one linear-combination term {variable, coefficient word} shared by the witness kernel and the R1CS
-// mat-vec (both walk LCs of the same circuit; the coefficient words are built by engine.cu: do_open).
+// mat-vec (both walk LCs of the same circuit; the coefficient words are built by witness_program.cpp: coef_words).
 #pragma once
 #include "ff.cuh"
 

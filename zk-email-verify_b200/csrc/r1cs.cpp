@@ -126,7 +126,7 @@ Circuit read_r1cs(const uint8_t* b, size_t len) {
     if (c.coefs.size() >= (1u << 24)) throw std::runtime_error(".r1cs has more than 2^24 distinct coefficients");
 
     // Powers of two (+-2^k) right after 1 and r - 1, so that they get the small table indices the engine's shift
-    // shortcut needs (engine.cu: do_open); every other coefficient after them, each group in order of appearance.
+    // shortcut needs (witness_program.cpp: coef_words); every other coefficient after them, each group in order of appearance.
     {
         std::vector<uint32_t> order = {0, 1};
         for (int pass = 0; pass < 2; ++pass)

@@ -30,6 +30,10 @@ class CircuitInfo(ctypes.Structure):
         "n_levels", "n_ops", "n_coefs", "domain_log2", "n_groups")] + [(n, c_u64) for n in ("nnz_a", "nnz_b", "nnz_c")]
 
 
+class ProgramStats(ctypes.Structure):
+    _fields_ = [(n, c_u32) for n in ("n_levels", "n_iters", "n_ops_kept", "n_coop_ops", "n_terms", "cluster")] + [("digest", c_u64)]
+
+
 def _sig(name, restype, argtypes):
     fn = getattr(lib, name)
     fn.restype = restype
@@ -47,6 +51,8 @@ zke_circuit_group = _sig("zke_circuit_group", c_int, [c_void_p, c_u32, c_char_p,
 zke_circuit_input_offset = _sig("zke_circuit_input_offset", c_i64, [c_void_p, c_char_p, ctypes.POINTER(c_u32)])
 zke_circuit_array = _sig("zke_circuit_array", c_void_p, [c_void_p, c_int, ctypes.POINTER(c_size_t)])
 zke_circuit_scope_name = _sig("zke_circuit_scope_name", c_char_p, [c_void_p, c_u32])
+zke_circuit_program_stats = _sig("zke_circuit_program_stats", c_int, [c_void_p, c_int, c_int, c_int, c_u32, ctypes.POINTER(ProgramStats),
+                                                                      ctypes.POINTER(c_u32), c_size_t, c_char_p, c_size_t])
 zke_device_count = _sig("zke_device_count", c_int, [])
 zke_version = _sig("zke_version", c_char_p, [])
 

@@ -109,6 +109,23 @@ class Circuit:
         p = L.zke_circuit_array(self._h, which, ctypes.byref(n))
         return p, n.value
 
+    def program_stats(self, native_sha=True, native_regex=True, coop_fpmul=True, cluster=1) -> dict:
+        """What the engine's lowering of the witness program (csrc/witness_program.cpp) builds for these options, computed
+        on the host: the fields of zke_program_stats plus `level_ops`, the records per level that are not cooperative ops."""
+        st, err = L.ProgramStats(), ctypes.create_string_buffer(L.ERRCAP)
+        cap = max(1, self.info.n_levels)
+        while True:                # the first min(n_levels, cap) levels are written: once more if the program got deeper
+            level_ops = (L.c_u32 * cap)()
+            if L.zke_circuit_program_stats(self._h, int(native_sha), int(native_regex), int(coop_fpmul), cluster, ctypes.byref(st),
+                                           level_ops, cap, err, L.ERRCAP) != 0:
+                raise L.ZkeError(err.value.decode())
+            if st.n_levels <= cap:
+                break
+            cap = st.n_levels
+        out = {name: getattr(st, name) for name, _ in st._fields_}
+        out["level_ops"] = list(level_ops[:st.n_levels])
+        return out
+
     def scope_name(self, idx: int) -> str:
         s = L.zke_circuit_scope_name(self._h, idx)
         return s.decode() if s else "?"
