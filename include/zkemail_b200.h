@@ -50,6 +50,17 @@ zke_circuit* zke_circuit_build(const char* template_name, const int64_t* params,
  * Signals: input msg[msg_len], outputs out (match flag) and reveal0[msg_len]. */
 zke_circuit* zke_circuit_build_regex(const char* const* parts, const uint8_t* is_public, size_t n_parts, uint32_t msg_len,
                                      char* err, size_t errcap);
+/* An email app circuit from a JSON spec (the "write the regex, wrap EmailVerifier, reveal what it matched" recipe of the
+ * zk-email usage guide): the EmailVerifier body with its flags (maxHeadersLength,
+ * maxBodyLength, n, k, ignoreBodyHashCheck, enableHeaderMasking, enableBodyMasking, removeSoftLineBreaks, publicPubkey,
+ * regexStyle) plus exposeHeaderHash (default true: shaHi / shaLo are outputs), then per entry of `regexes` ({name,
+ * location: "header" | "body", parts: [{regexDef, isPublic, maxLength}]}) a regex that must match and, per public part, a
+ * PackRegexReveal output (`name`, or `name0`, `name1`, ... for several public parts) with its private index input
+ * (`nameIndex` / `name0Index`, ...); `externalInputs` ([{name, maxLength?}]) are public inputs, one field element or
+ * ceil(maxLength / 31) packed ones; `emailNullifier` adds the EmailNullifier output.  Signal order: outputs (pubkeyHash,
+ * shaHi, shaLo, masks, regex outputs, emailNullifier), public inputs (external inputs, pubkey if public), the
+ * EmailVerifier inputs, then the index inputs.  A malformed spec is refused with a message naming the field. */
+zke_circuit* zke_circuit_build_app(const char* spec_json, char* err, size_t errcap);
 void zke_circuit_free(zke_circuit* c);
 /* circom's constraint system: an iden3 `.r1cs` image (what `circom --r1cs` writes and `snarkjs r1cs info` / `snarkjs groth16
  * setup` read, /root/reference/docs/zk-email-docs/UsageGuide/README.md steps 3-5; layout in r1cs.cpp), BN254 only.  The
@@ -98,8 +109,9 @@ enum {
     ZKE_ARR_SHA_BLOCKS = 17, /* uint32: {n_blocks, per block: var_begin, var_end, temp_begin, temp_end, n_desc,
                                inputs[768], desc[n_desc][2] = {signal, quantity << 8 | bit}} - the Sha256compression
                                instances the engine evaluates natively (one compression instead of ~320 levels)  */
-    ZKE_ARR_REGEX_SEEDS = 18 /* uint32: {n_seeds, per seed: n_desc, n_bytes, n_states | mode << 31, first_mask lo, hi,
-                               bytes[n_bytes] (signal of message byte j), table[n_states * 64] (destination state of
+    ZKE_ARR_REGEX_SEEDS = 18 /* uint32: {n_seeds, per seed: n_desc, n_bytes, n_states | wide << 30 | mode << 31,
+                               first_mask lo, hi (wide = zk-regex shape with 65..255 states: 8 words, the 256-bit live set
+                               from its low word up), bytes[n_bytes] (signal of message byte j), table[n_states * 64] (destination state of
                                (source, byte), 0xff = none, 4 per word), mode 1 (compact shape): group[n_states * 64] (the
                                product that fires), desc[n_desc][2] = {signal, position << 8 | state or product}} - the
                                regex instances whose chained signals the engine seeds with one automaton run      */

@@ -7,6 +7,7 @@
 #include "../../include/zkemail_b200.h"
 #include "engine.hpp"
 #include "ec_host.hpp"
+#include "gadgets.hpp"
 #include <cstring>
 #include <memory>
 #include <random>
@@ -172,6 +173,111 @@ void flatten_values(const JV& v, std::vector<U256>& out) {
     while (u256_cmp(x, fr_params().p) >= 0) u256_sub(x, x, fr_params().p);
     if (neg && !x.is_zero()) u256_sub(x, fr_params().p, x);
     out.push_back(x);
+}
+
+// ---- email app spec (zke_circuit_build_app) ----
+void only_keys(const JV& o, const std::string& field, std::initializer_list<const char*> keys) {
+    if (o.type != JV::OBJ) throw std::runtime_error(field + ": expected an object");
+    for (auto& kv : o.obj) {
+        bool known = false;
+        for (const char* k : keys) known = known || kv.first == k;
+        if (!known) throw std::runtime_error(field + ": unknown key '" + kv.first + "'");
+    }
+}
+bool bool_of(const JV& o, const char* key, bool dflt, const std::string& field) {
+    const JV* v = o.get(key);
+    if (!v) return dflt;
+    if (v->type == JV::BOOL) return v->s == "true";
+    if (v->type == JV::NUM && (v->s == "0" || v->s == "1")) return v->s == "1";
+    throw std::runtime_error(field + key + ": expected true or false");
+}
+uint32_t uint_of(const JV& v, const std::string& field) {
+    if (v.type != JV::NUM || v.s.empty() || v.s.size() > 9 || v.s.find_first_not_of("0123456789") != std::string::npos)
+        throw std::runtime_error(field + ": expected a non-negative integer");
+    return (uint32_t)std::stoul(v.s);
+}
+std::string str_of(const JV& o, const char* key, const std::string& field) {
+    const JV* v = o.get(key);
+    if (!v) throw std::runtime_error(field + key + ": missing");
+    if (v->type != JV::STR) throw std::runtime_error(field + key + ": expected a string");
+    return v->s;
+}
+const JV* array_of(const JV& o, const char* key) {
+    const JV* v = o.get(key);
+    if (v && v->type != JV::ARR) throw std::runtime_error(std::string(key) + ": expected an array");
+    return v;
+}
+
+// a packed external input is ceil(maxLength / 31) public inputs, each a row of the verifier's IC: 64 KiB is 2,115 of them
+const uint32_t MAX_EXTERNAL_BYTES = 1u << 16;
+
+gadgets::AppSpec app_spec_of(const JV& s) {
+    only_keys(s, "spec", {"maxHeadersLength", "maxBodyLength", "n", "k", "ignoreBodyHashCheck", "enableHeaderMasking",
+                          "enableBodyMasking", "removeSoftLineBreaks", "publicPubkey", "regexStyle", "exposeHeaderHash",
+                          "regexes", "externalInputs", "emailNullifier", "shaPrecomputeSelector"});
+    gadgets::AppSpec a;
+    gadgets::EmailVerifierParams& ev = a.ev;
+    if (const JV* v = s.get("maxHeadersLength")) ev.max_headers_length = uint_of(*v, "maxHeadersLength");
+    if (const JV* v = s.get("maxBodyLength")) ev.max_body_length = uint_of(*v, "maxBodyLength");
+    if (const JV* v = s.get("n")) ev.n = uint_of(*v, "n");
+    if (const JV* v = s.get("k")) ev.k = uint_of(*v, "k");
+    if (ev.max_headers_length > (1u << 20) || ev.max_body_length > (1u << 20)) throw std::runtime_error("maxHeadersLength / maxBodyLength: at most 2^20");
+    if (ev.k > 64) throw std::runtime_error("k: at most 64");
+    ev.ignore_body_hash_check = bool_of(s, "ignoreBodyHashCheck", false, "");
+    ev.enable_header_masking = bool_of(s, "enableHeaderMasking", false, "");
+    ev.enable_body_masking = bool_of(s, "enableBodyMasking", false, "");
+    ev.remove_soft_line_breaks = bool_of(s, "removeSoftLineBreaks", false, "");
+    ev.public_pubkey = bool_of(s, "publicPubkey", false, "");
+    if (const JV* v = s.get("regexStyle")) {
+        const uint32_t st = uint_of(*v, "regexStyle");
+        if (st > 1) throw std::runtime_error("regexStyle: 0 (zk-regex shape) or 1 (compact shape)");
+        ev.regex_style = (int)st;
+    }
+    if (const JV* v = s.get("shaPrecomputeSelector"))   // input generation only (generate_app_inputs)
+        if (v->type != JV::STR && v->type != JV::NUL) throw std::runtime_error("shaPrecomputeSelector: expected a string");
+    a.expose_header_hash = bool_of(s, "exposeHeaderHash", true, "");
+    a.email_nullifier = bool_of(s, "emailNullifier", false, "");
+    if (const JV* rs = array_of(s, "regexes")) {
+        for (size_t r = 0; r < rs->arr.size(); ++r) {
+            const JV& e = rs->arr[r];
+            const std::string f = "regexes[" + std::to_string(r) + "].";
+            only_keys(e, "regexes[" + std::to_string(r) + "]", {"name", "location", "parts"});
+            gadgets::AppRegex rx;
+            rx.name = str_of(e, "name", f);
+            const std::string loc = str_of(e, "location", f);
+            if (loc != "header" && loc != "body") throw std::runtime_error(f + "location: '" + loc + "' is neither \"header\" nor \"body\"");
+            rx.body = loc == "body";
+            const JV* parts = e.get("parts");
+            if (!parts || parts->type != JV::ARR) throw std::runtime_error(f + "parts: expected an array");
+            for (size_t i = 0; i < parts->arr.size(); ++i) {
+                const JV& pt = parts->arr[i];
+                const std::string pf = f + "parts[" + std::to_string(i) + "]";
+                only_keys(pt, pf, {"regexDef", "isPublic", "maxLength"});
+                gadgets::AppRegexPart part;
+                part.regex = str_of(pt, "regexDef", pf + ".");
+                part.is_public = bool_of(pt, "isPublic", false, pf + ".");
+                if (const JV* ml = pt.get("maxLength")) part.max_length = uint_of(*ml, pf + ".maxLength");
+                rx.parts.push_back(part);
+            }
+            a.regexes.push_back(rx);
+        }
+    }
+    if (const JV* es = array_of(s, "externalInputs")) {
+        for (size_t i = 0; i < es->arr.size(); ++i) {
+            const std::string f = "externalInputs[" + std::to_string(i) + "]";
+            only_keys(es->arr[i], f, {"name", "maxLength"});
+            gadgets::AppExternalInput ei;
+            ei.name = str_of(es->arr[i], "name", f + ".");
+            if (const JV* ml = es->arr[i].get("maxLength")) {
+                ei.max_length = uint_of(*ml, f + ".maxLength");
+                if (ei.max_length == 0) throw std::runtime_error(f + ".maxLength: must be positive (leave it out for one field element)");
+                if (ei.max_length > MAX_EXTERNAL_BYTES)
+                    throw std::runtime_error(f + ".maxLength: at most " + std::to_string(MAX_EXTERNAL_BYTES) + " bytes");
+            }
+            a.external_inputs.push_back(ei);
+        }
+    }
+    return a;
 }
 
 }  // namespace
@@ -348,6 +454,19 @@ int zke_zkey_vkey_json(const zke_zkey* z, char* out, size_t* len) {
         s += "]}";
         return copy_out(s, out, len);
     } catch (const std::exception&) { return -1; }
+}
+
+zke_circuit* zke_circuit_build_app(const char* spec_json, char* err, size_t errcap) {
+    try {
+        if (!spec_json) throw std::runtime_error("null spec");
+        const gadgets::AppSpec spec = app_spec_of(JParser(spec_json).parse());
+        zke_circuit* c = new zke_circuit();
+        try { c->c = gadgets::build_email_app(spec); } catch (...) { delete c; throw; }
+        return c;
+    } catch (const std::exception& e) {
+        set_err(err, errcap, e.what());
+        return nullptr;
+    }
 }
 
 /* snarkjs input JSON -> packed [n_inputs][32] vector in witness order.  Mirrors circom_runtime's checks:

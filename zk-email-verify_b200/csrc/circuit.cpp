@@ -245,8 +245,8 @@ bool Builder::default_fuse_shrand() {
 
 // flat image of one RegexSeed (circuit.hpp); also what the engine appends to the device program's aux table
 void append_regex_seed(std::vector<uint32_t>& out, const RegexSeed& R) {
-    out.insert(out.end(), {(uint32_t)(R.desc.size() / 2), (uint32_t)R.bytes.size(), R.n_states | (R.mode << 31),
-                           (uint32_t)R.first_mask, (uint32_t)(R.first_mask >> 32)});
+    out.insert(out.end(), {(uint32_t)(R.desc.size() / 2), (uint32_t)R.bytes.size(), R.n_states | ((uint32_t)R.wide() << 30) | (R.mode << 31)});
+    for (int q = 0; q < (R.wide() ? 4 : 1); ++q) out.insert(out.end(), {(uint32_t)R.first_mask[q], (uint32_t)(R.first_mask[q] >> 32)});
     out.insert(out.end(), R.bytes.begin(), R.bytes.end());
     auto pack = [&](const std::vector<uint8_t>& t) {
         for (uint32_t q = 0; q < R.n_states * 64; ++q) {

@@ -99,10 +99,10 @@ enum ShaQuantity : uint32_t {
 // The witness program keeps all of its ops - the seeded signals are simply written twice with the same value, and the
 // CPU oracle walks the program as it is (witness_program.cpp uses the record when it levelises the program).
 struct RegexSeed {
-    uint32_t n_states = 0;            // <= 64
+    uint32_t n_states = 0;            // <= 255; more than 64 (mode 0) is the wide mode: a 256-bit live set
     std::vector<uint32_t> bytes;      // the variable holding message byte j (position j + 1 of the circuit; position 0 is the marker)
     std::vector<uint8_t> table;       // n_states x 256: destination of (source state, byte) or 0xff; byte 255 never fires
-    uint64_t first_mask = 1;          // live states after the marker position (bit 0 = state 0, always live)
+    uint64_t first_mask[4] = {1, 0, 0, 0};   // live states after the marker position (bit 0 = state 0, always live)
     std::vector<uint32_t> desc;       // 2 words per seeded signal: {variable, position << 8 | state}, position >= 1
     // mode 1 - the compact shape (regex.cpp: regex_circuit_compact): ONE state per position (the automaton of live-state
     // sets is deterministic, n_states <= 255, first_mask = the state after the marker), the chain runs through the `fire`
@@ -110,6 +110,7 @@ struct RegexSeed {
     // descriptor {variable, position << 8 | product id} is 1 exactly when that product fires at that position.
     uint32_t mode = 0;
     std::vector<uint8_t> group;       // mode 1: n_states x 256
+    bool wide() const { return mode == 0 && n_states > 64; }
 };
 
 void append_regex_seed(std::vector<uint32_t>& out, const RegexSeed& R);   // flat image (circuit.cpp)
@@ -152,8 +153,8 @@ struct Circuit {
     std::vector<uint32_t> sha_flat;
 
     std::vector<RegexSeed> regex_seeds; // zk-regex instances whose state signals can be produced by an automaton run (may be empty)
-    // flat image of regex_seeds: {n_seeds, then per seed: n_desc, n_bytes, n_states | mode << 31, first_mask lo, hi,
-    // bytes[n_bytes], table[n_states * 64] (4 bytes per word, little-endian), mode 1: group[n_states * 64], desc[2 n_desc]}
+    // flat image of regex_seeds: {n_seeds, then per seed: n_desc, n_bytes, n_states | wide << 30 | mode << 31, first_mask
+    // lo, hi (wide: 8 words, the 256-bit mask from its low word up), bytes[n_bytes], table[n_states * 64] (4 bytes per word, little-endian), mode 1: group[n_states * 64], desc[2 n_desc]}
     // (built by finalize; ZKE_ARR_REGEX_SEEDS); the engine appends the same image to the program's aux table
     std::vector<uint32_t> regex_flat;
 

@@ -886,28 +886,103 @@ LC remove_soft_line_breaks(Builder& b, const LCVec& encoded, const LCVec& decode
 
 // ---------------------------------------------------------------- email-verifier.circom
 Circuit build_email_verifier(const EmailVerifierParams& P, bool materialize_linear) {
+    AppSpec app;
+    app.ev = P;
+    if (P.twitter) {
+        // Proof-of-Twitter: `email was meant for @(\w+)` in the body, PackRegexReveal(maxBodyLength, 21), public address
+        if (P.ignore_body_hash_check) throw std::runtime_error("TwitterVerifier needs the body (ignoreBodyHashCheck = 0)");
+        app.expose_header_hash = false;     // EV.shaHi / EV.shaLo: signals of the sub-component
+        app.scope = "TwitterVerifier";
+        AppRegex rx;
+        rx.name = "twitterUsername";
+        rx.body = true;
+        rx.scope = "TwitterResetRegex";
+        rx.parts = {{"email was meant for @", false, 0}, {"[a-zA-Z0-9_]+", true, 21}};
+        app.regexes.push_back(rx);
+        app.external_inputs.push_back({"address", 0});   // component main { public [ address ] }
+    }
+    return build_email_app(app, materialize_linear);
+}
+
+// every signal name EmailVerifier (or the app wrapper) declares under any flag; an app's names must avoid them
+static const char* const EMAIL_VERIFIER_SIGNALS[] = {
+    "pubkeyHash", "shaHi", "shaLo", "maskedHeader", "maskedBody", "emailHeader", "emailHeaderLength", "pubkey", "signature",
+    "headerMask", "bodyHashIndex", "precomputedSHA", "emailBody", "emailBodyLength", "decodedEmailBodyIn", "bodyMask",
+    "emailNullifier"};
+
+static uint32_t packed_len(uint32_t bytes) { return (bytes + 30) / 31; }   // computeIntChunkLength (utils/bytes.circom:10-20)
+
+Circuit build_email_app(const AppSpec& A, bool materialize_linear) {
+    const EmailVerifierParams& P = A.ev;
     const uint32_t H = P.max_headers_length, Bd = P.max_body_length, n = P.n, k = P.k;
     if (H % 64 != 0 || Bd % 64 != 0 || !(n * k > 2048) || !(n < 127))
         throw std::runtime_error("EmailVerifier: parameter asserts failed (email-verifier.circom:43-46)");
+
+    // the app's signal names: unique, and none of EmailVerifier's
+    std::vector<std::string> taken;
+    auto claim = [&](const std::string& field, const std::string& name) {
+        if (name.empty()) throw std::runtime_error(field + ": empty name");
+        for (const char* r : EMAIL_VERIFIER_SIGNALS)
+            if (name == r) throw std::runtime_error(field + ": signal name '" + name + "' collides with an EmailVerifier signal");
+        for (const std::string& t : taken)
+            if (t == name) throw std::runtime_error(field + ": signal name '" + name + "' is used twice");
+        taken.push_back(name);
+    };
+    struct Reveal { std::string out, index; uint32_t max_length; };
+    std::vector<std::vector<Reveal>> reveals(A.regexes.size());
+    for (size_t r = 0; r < A.regexes.size(); ++r) {
+        const AppRegex& rx = A.regexes[r];
+        const std::string field = "regexes[" + std::to_string(r) + "]";
+        if (rx.name.empty()) throw std::runtime_error(field + ".name: empty name");
+        if (rx.parts.empty()) throw std::runtime_error(field + ".parts: no parts");
+        if (rx.body && P.ignore_body_hash_check)
+            throw std::runtime_error(field + ".location: a body regex needs the body (ignoreBodyHashCheck is set)");
+        const uint32_t searched = rx.body ? Bd : H;
+        uint32_t n_pub = 0;
+        for (auto& pt : rx.parts) n_pub += pt.is_public ? 1 : 0;
+        uint32_t q = 0;
+        for (size_t i = 0; i < rx.parts.size(); ++i) {
+            const AppRegexPart& pt = rx.parts[i];
+            if (!pt.is_public) continue;
+            const std::string pf = field + ".parts[" + std::to_string(i) + "].maxLength";
+            if (pt.max_length == 0) throw std::runtime_error(pf + ": a public part needs maxLength");
+            if (pt.max_length > searched)
+                throw std::runtime_error(pf + ": " + std::to_string(pt.max_length) + " is larger than the searched " +
+                                         (rx.body ? "body" : "header") + " (" + std::to_string(searched) + " bytes)");
+            const std::string base = n_pub == 1 ? rx.name : rx.name + std::to_string(q);
+            reveals[r].push_back(Reveal{base, base + "Index", pt.max_length});
+            ++q;
+        }
+    }
+    for (size_t r = 0; r < A.regexes.size(); ++r) {
+        const std::string field = "regexes[" + std::to_string(r) + "].name";
+        if (reveals[r].empty()) claim(field, A.regexes[r].name);      // no signal of its own, but the name stays unique
+        for (auto& rv : reveals[r]) { claim(field, rv.out); claim(field, rv.index); }
+    }
+    for (size_t e = 0; e < A.external_inputs.size(); ++e) claim("externalInputs[" + std::to_string(e) + "].name", A.external_inputs[e].name);
+
     Builder b("EmailVerifier");
     b.materialize_linear = materialize_linear;
     if (P.regex_style >= 0) b.regex_style = P.regex_style;
     ScopeGuard g(b, "EmailVerifier");
 
     // outputs first (circom witness order)
-    if (P.twitter && P.ignore_body_hash_check) throw std::runtime_error("TwitterVerifier needs the body (ignoreBodyHashCheck = 0)");
     Var pubkey_hash = b.declare_outputs("pubkeyHash", 1)[0];
-    Var sha_hi = 0, sha_lo = 0, twitter_username = 0;
-    if (P.twitter) twitter_username = b.declare_outputs("twitterUsername", 1)[0];
-    else { sha_hi = b.declare_outputs("shaHi", 1)[0]; sha_lo = b.declare_outputs("shaLo", 1)[0]; }
+    Var sha_hi = 0, sha_lo = 0;
+    if (A.expose_header_hash) { sha_hi = b.declare_outputs("shaHi", 1)[0]; sha_lo = b.declare_outputs("shaLo", 1)[0]; }
     std::vector<Var> masked_header, masked_body;
     if (P.enable_header_masking) masked_header = b.declare_outputs("maskedHeader", H);
     if (!P.ignore_body_hash_check && P.enable_body_masking) masked_body = b.declare_outputs("maskedBody", Bd);
+    std::vector<std::vector<std::vector<Var>>> reveal_out(A.regexes.size());
+    for (size_t r = 0; r < A.regexes.size(); ++r)
+        for (auto& rv : reveals[r]) reveal_out[r].push_back(b.declare_outputs(rv.out, packed_len(rv.max_length)));
+    Var nullifier = 0;
+    if (A.email_nullifier) nullifier = b.declare_outputs("emailNullifier", 1)[0];
 
     auto to_lcs = [](const std::vector<Var>& v) { LCVec o(v.size()); for (size_t i = 0; i < v.size(); ++i) o[i] = LC(v[i]); return o; };
+    // public inputs: the app's external inputs, bound to the proof through their public-input rows of the QAP (SURVEY A.7)
+    for (auto& ei : A.external_inputs) b.declare_inputs(ei.name, ei.max_length ? packed_len(ei.max_length) : 1, true);
     std::vector<Var> pubkey_v;
-    LC twitter_address;
-    if (P.twitter) twitter_address = LC(b.declare_inputs("address", 1, true)[0]);   // component main { public [ address ] }
     if (P.public_pubkey) pubkey_v = b.declare_inputs("pubkey", k, true);
     LCVec email_header = to_lcs(b.declare_inputs("emailHeader", H, false));
     LC email_header_length = LC(b.declare_inputs("emailHeaderLength", 1, false)[0]);
@@ -924,15 +999,16 @@ Circuit build_email_verifier(const EmailVerifierParams& P, bool materialize_line
         if (P.remove_soft_line_breaks) decoded_in = to_lcs(b.declare_inputs("decodedEmailBodyIn", Bd, false));
         if (P.enable_body_masking) body_mask = to_lcs(b.declare_inputs("bodyMask", Bd, false));
     }
-    LC twitter_index;
-    if (P.twitter) twitter_index = LC(b.declare_inputs("twitterUsernameIndex", 1, false)[0]);
+    std::vector<std::vector<LC>> reveal_index(A.regexes.size());
+    for (size_t r = 0; r < A.regexes.size(); ++r)
+        for (auto& rv : reveals[r]) reveal_index[r].push_back(LC(b.declare_inputs(rv.index, 1, false)[0]));
 
     num2bits(b, email_header_length, log2_ceil(H));                      // :58-59
     assert_zero_padding(b, email_header, email_header_length);           // :63
     LCVec sha = sha256_bytes(b, email_header, email_header_length);      // :67
     LCVec packed = pack_bits(b, sha, 128);                               // :68-71
-    if (P.twitter) { b.signal(packed[0]); b.signal(packed[1]); }          // EV.shaHi / EV.shaLo: signals of the sub-component
-    else { b.assign_output(sha_hi, packed[0]); b.assign_output(sha_lo, packed[1]); }
+    if (A.expose_header_hash) { b.assign_output(sha_hi, packed[0]); b.assign_output(sha_lo, packed[1]); }
+    else { b.signal(packed[0]); b.signal(packed[1]); }
 
     const uint32_t rsa_message_size = (256 + n) / n;                     // :74-84
     LCVec rsa_message(k);
@@ -975,15 +1051,28 @@ Circuit build_email_verifier(const EmailVerifierParams& P, bool materialize_line
         }
     }
     b.assign_output(pubkey_hash, poseidon_large(b, n, pubkey));          // :173
-    if (P.twitter) {
-        ScopeGuard tg(b, "TwitterVerifier");
-        LCVec rx = twitter_reset_regex(b, email_body);
-        b.enforce_eq(rx[0], one_lc());                                   // twitterFound === 1
-        LCVec reveal(rx.begin() + 1, rx.end());
-        LCVec packs = pack_regex_reveal(b, reveal, twitter_index, 21);   // maxTwitterUsernameLength = 21 -> one field element
-        b.assign_output(twitter_username, packs[0]);
-        (void)twitter_address;   // bound to the proof through its public-input row of the QAP (SURVEY A.7)
+    if (A.regexes.empty() && !A.email_nullifier) return b.finalize();
+
+    ScopeGuard ag(b, A.scope);
+    for (size_t r = 0; r < A.regexes.size(); ++r) {                      // the app's regexes (UsageGuide step 2)
+        const AppRegex& ar = A.regexes[r];
+        const LCVec& msg = ar.body ? (P.remove_soft_line_breaks ? decoded_in : email_body) : email_header;
+        std::vector<std::pair<std::string, bool>> parts;
+        for (auto& pt : ar.parts) parts.emplace_back(pt.regex, pt.is_public);
+        LCVec rx;
+        try {
+            rx = regex_match_reveals(b, ar.scope.empty() ? ar.name : ar.scope, parts, msg);
+        } catch (const std::exception& e) {
+            throw std::runtime_error("regexes[" + std::to_string(r) + "] (" + ar.name + "): " + e.what());
+        }
+        b.enforce_eq(rx[0], one_lc());                                   // the regex must match
+        for (size_t q = 0; q < reveals[r].size(); ++q) {
+            LCVec reveal(rx.begin() + 1 + q * msg.size(), rx.begin() + 1 + (q + 1) * msg.size());
+            LCVec packs = pack_regex_reveal(b, reveal, reveal_index[r][q], reveals[r][q].max_length);
+            for (size_t i = 0; i < packs.size(); ++i) b.assign_output(reveal_out[r][q][i], packs[i]);
+        }
     }
+    if (A.email_nullifier) b.assign_output(nullifier, email_nullifier(b, n, signature));   // helpers/email-nullifier.circom
     return b.finalize();
 }
 

@@ -94,5 +94,31 @@ struct EmailVerifierParams {
 };
 Circuit build_email_verifier(const EmailVerifierParams& p, bool materialize_linear = true);
 
+// zk-regex circuit with one reveal array per public part: out = [match, reveal of public part 0 (msg.size()), reveal of
+// public part 1, ...] (regex_match ORs every public part into one reveal array)
+LCVec regex_match_reveals(Builder& b, const std::string& scope, const std::vector<std::pair<std::string, bool>>& parts, const LCVec& msg);
+
+// ---- email app circuits: EmailVerifier + the app's regexes, revealed substrings and public inputs ----------------------
+// The circuit a zk-email app writes by hand (docs/zk-email-docs/UsageGuide/README.md: write the regex, wrap EmailVerifier,
+// reveal what it matched), built from a description.  TwitterVerifier is the app {body regex twitterUsername, external
+// input address, exposeHeaderHash = false}; EmailVerifier is the app with nothing added.
+struct AppRegexPart { std::string regex; bool is_public = false; uint32_t max_length = 0; };   // max_length: public parts
+struct AppRegex {
+    std::string name;
+    bool body = false;                 // search emailBody (decodedEmailBodyIn with removeSoftLineBreaks), else emailHeader
+    std::vector<AppRegexPart> parts;
+    std::string scope;                 // scope of its constraints (default: name)
+};
+struct AppExternalInput { std::string name; uint32_t max_length = 0; };   // 0: one field element, else PackBytes layout
+struct AppSpec {
+    EmailVerifierParams ev;            // ev.twitter is ignored
+    bool expose_header_hash = true;
+    std::vector<AppRegex> regexes;
+    std::vector<AppExternalInput> external_inputs;
+    bool email_nullifier = false;
+    std::string scope = "EmailApp";    // scope of everything after pubkeyHash
+};
+Circuit build_email_app(const AppSpec& spec, bool materialize_linear = true);
+
 }  // namespace gadgets
 }  // namespace zke

@@ -9,7 +9,8 @@
 // DFA, then the zk-regex circuit shape: the input is prefixed with byte 255 (the `^` marker), state 0 is
 // live at every position (unanchored search), states[i+1][s] is the OR over incoming transitions of
 // (states[i][src] AND in[i] in class), out = OR_i states[i][accept], and reveal[i] = in[i] wherever a
-// transition of the public part fires (contract in SURVEY A.6).
+// transition of the public part fires (contract in SURVEY A.6).  regex_match_reveals gives every public part a reveal
+// array of its own (the edges of public part p carry tag bit p); the other entry points OR all public parts into reveal0.
 //
 // Builder::regex_style = 1 emits the same function of the input (same `out`, same `reveal0`) in a different circuit
 // shape ("compact", regex_circuit_compact below): character classes from nibble one-hots of a single bit decomposition per
@@ -34,12 +35,12 @@ namespace {
 
 typedef std::bitset<256> CharSet;
 
-struct NfaEdge { int to; CharSet cs; bool eps; bool pub; };
+struct NfaEdge { int to; CharSet cs; bool eps; uint32_t pub; };   // pub: bit set of the public parts the edge belongs to
 struct Nfa {
     std::vector<std::vector<NfaEdge>> adj;
     int new_state() { adj.emplace_back(); return (int)adj.size() - 1; }
-    void eps(int a, int b) { adj[a].push_back(NfaEdge{b, CharSet(), true, false}); }
-    void chr(int a, int b, const CharSet& cs, bool pub) { adj[a].push_back(NfaEdge{b, cs, false, pub}); }
+    void eps(int a, int b) { adj[a].push_back(NfaEdge{b, CharSet(), true, 0}); }
+    void chr(int a, int b, const CharSet& cs, uint32_t pub) { adj[a].push_back(NfaEdge{b, cs, false, pub}); }
 };
 struct Frag { int s, e; };
 
@@ -48,8 +49,8 @@ struct Parser {
     const std::string& re;
     size_t pos = 0;
     Nfa& nfa;
-    bool pub;
-    Parser(const std::string& r, Nfa& n, bool p) : re(r), nfa(n), pub(p) {}
+    uint32_t pub;
+    Parser(const std::string& r, Nfa& n, uint32_t p) : re(r), nfa(n), pub(p) {}
 
     bool more() const { return pos < re.size(); }
     char peek() const { return re[pos]; }
@@ -193,19 +194,28 @@ struct Parser {
     }
 };
 
-struct DfaTransition { int src, dst; CharSet cs; bool pub; };
+struct DfaTransition { int src, dst; CharSet cs; uint32_t pub; };
 struct Dfa {
     int n_states = 0;
     std::vector<bool> accept;
     std::vector<DfaTransition> trans;   // grouped by (src, dst, pub)
 };
 
-Dfa build_dfa(const std::vector<std::pair<std::string, bool>>& parts) {
+// per_part = false: every public part carries tag 1 (one reveal array for all of them); true: public part p carries tag
+// 1 << p, so that each public part gets a reveal array of its own
+Dfa build_dfa(const std::vector<std::pair<std::string, bool>>& parts, bool per_part = false) {
     Nfa nfa;
     int start = nfa.new_state();
     int cur = start;
+    uint32_t n_public = 0;
     for (auto& pr : parts) {
-        Parser ps(pr.first, nfa, pr.second);
+        uint32_t tag = 0;
+        if (pr.second) {
+            if (per_part && n_public >= 32) throw std::runtime_error("regex: more than 32 public parts");
+            tag = per_part ? 1u << n_public : 1u;
+            ++n_public;
+        }
+        Parser ps(pr.first, nfa, tag);
         Frag f = ps.parse_alt();
         if (ps.more()) throw std::runtime_error("regex: trailing characters");
         nfa.eps(cur, f.s);
@@ -231,14 +241,14 @@ Dfa build_dfa(const std::vector<std::pair<std::string, bool>>& parts) {
         return id;
     };
     get(closure({start}));
-    std::map<std::tuple<int, int, bool>, CharSet> grouped;
+    std::map<std::tuple<int, int, uint32_t>, CharSet> grouped;
     for (size_t si = 0; si < sets.size(); ++si) {
         for (int c = 0; c < 256; ++c) {
             std::set<int> tgt;
-            bool pub = false;
+            uint32_t pub = 0;
             for (int u : sets[si])
                 for (auto& e : nfa.adj[u])
-                    if (!e.eps && e.cs.test(c)) { tgt.insert(e.to); pub = pub || e.pub; }
+                    if (!e.eps && e.cs.test(c)) { tgt.insert(e.to); pub |= e.pub; }
             if (tgt.empty()) continue;
             int ti = get(closure(tgt));
             grouped[std::make_tuple((int)si, ti, pub)].set(c);
@@ -263,7 +273,8 @@ LC range_match(Builder& b, const LC& in, int lo, int hi) {
 
 }  // namespace
 
-static LCVec regex_circuit(Builder& b, const Dfa& dfa, const LCVec& msg) {
+// out = [match, reveal of tag bit 0 (msg.size()), reveal of tag bit 1, ...]: n_reveal arrays (regex_match_reveals)
+static LCVec regex_circuit(Builder& b, const Dfa& dfa, const LCVec& msg, uint32_t n_reveal = 1) {
     const int S = dfa.n_states;
     const size_t num_bytes = msg.size() + 1;
     if (dfa.accept[0]) throw std::runtime_error("regex: matches the empty string");
@@ -287,10 +298,11 @@ static LCVec regex_circuit(Builder& b, const Dfa& dfa, const LCVec& msg) {
     LCVec states(S);                       // states[i][*]
     states[0] = one;
     LCVec accept_flags;
-    LCVec out(1 + msg.size());
-    // record for the device's automaton run (circuit.hpp: RegexSeed): possible when every message byte is a plain signal
+    LCVec out(1 + n_reveal * msg.size());
+    // record for the device's automaton run (circuit.hpp: RegexSeed): possible when every message byte is a plain signal;
+    // more than 64 states take the wide live set (256 bits), the uint8 table caps the DFA at 255 states
     RegexSeed seed;
-    bool seedable = S <= 64 && msg.size() < (1u << 24);
+    bool seedable = S <= 255 && msg.size() < (1u << 24);
     for (size_t j = 0; j < msg.size() && seedable; ++j) {
         Var v;
         if (msg[j].is_single_var(&v)) seed.bytes.push_back(v); else seedable = false;
@@ -301,7 +313,7 @@ static LCVec regex_circuit(Builder& b, const Dfa& dfa, const LCVec& msg) {
         for (size_t k = 0; k < dfa.trans.size(); ++k) {
             const DfaTransition& t = dfa.trans[k];
             for (int c = 0; c < 255; ++c) if (t.cs.test(c)) seed.table[(size_t)t.src * 256 + c] = (uint8_t)t.dst;
-            if (t.src == 0 && t.cs.test(255)) seed.first_mask |= 1ull << t.dst;      // the marker byte: only state 0 is live before it
+            if (t.src == 0 && t.cs.test(255)) seed.first_mask[t.dst >> 6] |= 1ull << (t.dst & 63);   // the marker byte: only state 0 is live before it
         }
     }
     for (size_t i = 0; i < num_bytes; ++i) {
@@ -335,10 +347,10 @@ static LCVec regex_circuit(Builder& b, const Dfa& dfa, const LCVec& msg) {
             for (int k : incoming[s]) if (!fire[k].is_zero()) ins.push_back(fire[k]);
             if (!ins.empty()) next[s] = multi_or(b, ins);
         }
-        if (!is_marker) {
+        for (uint32_t p = 0; p < n_reveal && !is_marker; ++p) {
             LCVec pubs;
-            for (size_t k = 0; k < dfa.trans.size(); ++k) if (dfa.trans[k].pub && !fire[k].is_zero()) pubs.push_back(fire[k]);
-            out[i] = pubs.empty() ? LC() : b.mul(in, multi_or(b, pubs));   // reveal0[i-1] <== in[i] * is_reveal
+            for (size_t k = 0; k < dfa.trans.size(); ++k) if ((dfa.trans[k].pub >> p & 1) && !fire[k].is_zero()) pubs.push_back(fire[k]);
+            out[p * msg.size() + i] = pubs.empty() ? LC() : b.mul(in, multi_or(b, pubs));   // reveal_p[i-1] <== in[i] * is_reveal
         }
         states.swap(next);
         if (seedable && !is_marker)
@@ -363,7 +375,7 @@ namespace {
 // {0}), their transitions on bytes 0..254 (byte 255 is the `^` marker and matches nothing inside the message), whether a
 // public edge is taken by some thread, and whether the set holds an accepting DFA state.
 struct PowerDfa {
-    struct Tr { int src, dst; CharSet cs; bool pub; };
+    struct Tr { int src, dst; CharSet cs; uint32_t pub; };
     std::vector<std::vector<int>> members;
     std::vector<bool> accept;
     std::vector<Tr> trans;            // only transitions with dst != 0 ("every thread died" needs no product)
@@ -372,10 +384,11 @@ struct PowerDfa {
 
 PowerDfa build_power(const Dfa& dfa) {
     const int S = dfa.n_states;
-    std::vector<std::array<int, 256>> delta(S);        // dst * 2 + pub, or -1
+    std::vector<std::array<int, 256>> delta(S);        // dst * 2 + (pub != 0), or -1
+    std::vector<std::array<uint32_t, 256>> pubs(S);    // public-part tags of the edge
     for (auto& row : delta) row.fill(-1);
     for (auto& t : dfa.trans)
-        for (int c = 0; c < 256; ++c) if (t.cs.test(c)) delta[t.src][c] = t.dst * 2 + (t.pub ? 1 : 0);
+        for (int c = 0; c < 256; ++c) if (t.cs.test(c)) { delta[t.src][c] = t.dst * 2 + (t.pub ? 1 : 0); pubs[t.src][c] = t.pub; }
     PowerDfa pd;
     std::map<std::vector<int>, int> index;
     auto get = [&](std::vector<int> set) {
@@ -389,19 +402,19 @@ PowerDfa build_power(const Dfa& dfa) {
         pd.members.push_back(set);
         return id;
     };
-    auto step = [&](const std::vector<int>& from, int c, bool& pub) {
+    auto step = [&](const std::vector<int>& from, int c, uint32_t& pub) {
         std::vector<int> to{0};
-        pub = false;
-        for (int s : from) if (delta[s][c] >= 0) { to.push_back(delta[s][c] >> 1); pub = pub || (delta[s][c] & 1); }
+        pub = 0;
+        for (int s : from) if (delta[s][c] >= 0) { to.push_back(delta[s][c] >> 1); pub |= pubs[s][c]; }
         return to;
     };
     get({0});
-    bool dummy;
+    uint32_t dummy;
     pd.after_marker = get(step({0}, 255, dummy));
-    std::map<std::tuple<int, int, bool>, CharSet> grouped;
+    std::map<std::tuple<int, int, uint32_t>, CharSet> grouped;
     for (size_t li = 0; li < pd.members.size(); ++li) {
         for (int c = 0; c < 255; ++c) {
-            bool pub;
+            uint32_t pub;
             const std::vector<int> from = pd.members[li];      // copy: get() may grow pd.members
             int ti = get(step(from, c, pub));
             if (ti != 0) grouped[std::make_tuple((int)li, ti, pub)].set(c);
@@ -464,12 +477,12 @@ LC class_match(Builder& b, const ByteOneHot& oh, const CharSet& cs, std::map<std
     return m;
 }
 
-LCVec regex_circuit_compact(Builder& b, const Dfa& dfa, const LCVec& msg) {
+LCVec regex_circuit_compact(Builder& b, const Dfa& dfa, const LCVec& msg, uint32_t n_reveal = 1) {
     if (dfa.accept[0]) throw std::runtime_error("regex: matches the empty string");
     const PowerDfa pd = build_power(dfa);
     const int S = (int)pd.members.size();
     if (getenv("ZKE_REGEX_DEBUG")) {
-        std::set<std::tuple<int, bool, std::string>> groups;
+        std::set<std::tuple<int, uint32_t, std::string>> groups;
         std::set<std::string> classes;
         for (auto& t : pd.trans) { groups.insert(std::make_tuple(t.dst, t.pub, t.cs.to_string())); classes.insert(t.cs.to_string()); }
         fprintf(stderr, "regex compact: %d DFA states, %d live sets, %zu transitions, %zu (dst, pub, class) groups, %zu classes\n",
@@ -481,10 +494,10 @@ LCVec regex_circuit_compact(Builder& b, const Dfa& dfa, const LCVec& msg) {
     LC accepted;                           // number of positions at which an accepting DFA state is live
     auto count_accepts = [&]() { for (int s = 0; s < S; ++s) if (pd.accept[s] && !states[s].is_zero()) accepted += states[s]; };
     count_accepts();
-    LCVec out(1 + msg.size());
+    LCVec out(1 + n_reveal * msg.size());
     // record for the device's automaton run (circuit.hpp: RegexSeed, mode 1): the chain runs through the `fire` products
     RegexSeed seed;
-    std::map<std::tuple<int, bool, std::string>, int> gid;           // (dst, public, class) -> product id, the same at every position
+    std::map<std::tuple<int, uint32_t, std::string>, int> gid;           // (dst, public, class) -> product id, the same at every position
     for (auto& t : pd.trans) gid.emplace(std::make_tuple(t.dst, t.pub, t.cs.to_string()), (int)gid.size());
     bool seedable = S <= 255 && gid.size() <= 254 && msg.size() < (1u << 24);
     for (size_t j = 0; j < msg.size() && seedable; ++j) {
@@ -494,7 +507,7 @@ LCVec regex_circuit_compact(Builder& b, const Dfa& dfa, const LCVec& msg) {
     if (seedable) {
         seed.mode = 1;
         seed.n_states = (uint32_t)S;
-        seed.first_mask = (uint64_t)pd.after_marker;
+        seed.first_mask[0] = (uint64_t)pd.after_marker;
         seed.table.assign((size_t)S * 256, 0xff);
         seed.group.assign((size_t)S * 256, 0xff);
         for (auto& t : pd.trans) {
@@ -505,11 +518,11 @@ LCVec regex_circuit_compact(Builder& b, const Dfa& dfa, const LCVec& msg) {
     for (size_t i = 0; i < msg.size(); ++i) {
         const ByteOneHot oh = byte_one_hot(b, msg[i]);
         std::map<std::pair<uint32_t, uint32_t>, LC> cache;
-        LCVec next(S);
-        LC reveal, moved;
+        LCVec next(S), reveal(n_reveal);
+        LC moved;
         // transitions that enter the same live set on the same class (and agree on `public`) share one product: the
         // states are one-hot, so the sum of their sources is itself 0 / 1
-        std::map<std::tuple<int, bool, std::string>, std::pair<LC, const CharSet*>> groups;
+        std::map<std::tuple<int, uint32_t, std::string>, std::pair<LC, const CharSet*>> groups;
         for (auto& t : pd.trans) {
             if (states[t.src].is_zero()) continue;                   // live set statically unreachable at this position
             auto& gr = groups[std::make_tuple(t.dst, t.pub, t.cs.to_string())];
@@ -529,10 +542,11 @@ LCVec regex_circuit_compact(Builder& b, const Dfa& dfa, const LCVec& msg) {
             if (seedable && fire.is_single_var(&fv)) { seed.desc.push_back(fv); seed.desc.push_back((uint32_t)((i + 1) << 8) | (uint32_t)gid[kv.first]); }
             next[std::get<0>(kv.first)] += fire;
             moved += fire;
-            if (std::get<1>(kv.first)) reveal += fire;
+            for (uint32_t p = 0; p < n_reveal; ++p) if (std::get<1>(kv.first) >> p & 1) reveal[p] += fire;
         }
         next[0] = one - moved;                                       // no transition fired: only the fresh thread is live
-        out[1 + i] = reveal.is_zero() ? LC() : b.mul(msg[i], reveal);   // reveal0[i] <== in[i] * is_reveal
+        for (uint32_t p = 0; p < n_reveal; ++p)                       // reveal_p[i] <== in[i] * is_reveal
+            out[1 + p * msg.size() + i] = reveal[p].is_zero() ? LC() : b.mul(msg[i], reveal[p]);
         states.swap(next);
         count_accepts();
     }
@@ -559,6 +573,14 @@ LCVec regex_match(Builder& b, const std::string& scope, const std::vector<std::p
     ScopeGuard g(b, scope.c_str());
     const Dfa dfa = build_dfa(parts);
     return b.regex_style ? regex_circuit_compact(b, dfa, msg) : regex_circuit(b, dfa, msg);
+}
+
+LCVec regex_match_reveals(Builder& b, const std::string& scope, const std::vector<std::pair<std::string, bool>>& parts, const LCVec& msg) {
+    ScopeGuard g(b, scope.c_str());
+    uint32_t n_public = 0;
+    for (auto& p : parts) n_public += p.second ? 1 : 0;
+    const Dfa dfa = build_dfa(parts, true);
+    return b.regex_style ? regex_circuit_compact(b, dfa, msg, n_public) : regex_circuit(b, dfa, msg, n_public);
 }
 
 LCVec twitter_reset_regex(Builder& b, const LCVec& msg) {

@@ -188,23 +188,27 @@ __device__ void sha_coop(const DevProgram& P, uint8_t* w, uint32_t aux_off, unsi
 // ---- zk-regex state seeding (circuit.hpp: RegexSeed) -------------------------------------------------------------------
 // The state signals of a zk-regex instance form a chain as long as the message (position i needs position i - 1); the
 // set of live DFA states per position is just an automaton run.  The CTA gathers the message bytes, one thread runs the
-// automaton (the live set is a 64-bit mask; state 0 is always live, byte 255 - the marker - fires nothing), and all
-// threads write the state signals of every position.  The instance's own ops follow at a handful of levels and write
-// the same values again; the CPU oracle walks only those, so "GPU witness == oracle witness" checks the seeding.
-// Shared buffer Q (SHA_Q_WORDS 64-bit words): masks of up to RX_CHUNK positions, then the staged bytes, carry at the end.
+// automaton (the live set is a 64-bit mask, or four of them in the wide mode for 65..255 states; state 0 is always live,
+// byte 255 - the marker - fires nothing), and all threads write the state signals of every position.  The instance's own
+// ops follow at a handful of levels and write the same values again; the CPU oracle walks only those, so "GPU witness ==
+// oracle witness" checks the seeding.
+// Shared buffer Q (SHA_Q_WORDS 64-bit words): the live sets of up to RX_CHUNK positions (RX_CHUNK / 4 in the wide mode,
+// four words each), then the staged bytes from word RX_CHUNK on, the carry in the last word (the last four, wide).
 static const uint32_t RX_CHUNK = 896;
+static_assert(RX_CHUNK + RX_CHUNK / 8 + 4 <= SHA_Q_WORDS, "regex chunk does not fit the shared buffer");
 __device__ void regex_coop(const DevProgram& P, uint8_t* w, uint32_t aux_off, unsigned long long* Q) {
     const uint32_t tid = threadIdx.x;
     const uint32_t* ax = P.aux + aux_off;
-    const uint32_t n_desc = ax[0], n_bytes = ax[1], n_states = ax[2] & 0x7fffffffu, mode = ax[2] >> 31;
+    const uint32_t n_desc = ax[0], n_bytes = ax[1], n_states = ax[2] & 0x3fffffffu, wide = (ax[2] >> 30) & 1u, mode = ax[2] >> 31;
     const unsigned long long first = (unsigned long long)ax[3] | ((unsigned long long)ax[4] << 32);
-    const uint32_t* bytes = ax + 5;
+    const uint32_t* bytes = ax + (wide ? 11 : 5);
     const uint8_t* table = reinterpret_cast<const uint8_t*>(bytes + n_bytes);
     const uint8_t* group = table + n_states * 256u;                  // mode 1 only
     const uint32_t* desc = bytes + n_bytes + n_states * 64 * (1 + mode);
+    const uint32_t chunk = wide ? RX_CHUNK / 4 : RX_CHUNK;
     uint8_t* staged = reinterpret_cast<uint8_t*>(Q + RX_CHUNK);
-    for (uint32_t base = 0; base < n_bytes; base += RX_CHUNK) {
-        const uint32_t cnt = min(RX_CHUNK, n_bytes - base);
+    for (uint32_t base = 0; base < n_bytes; base += chunk) {
+        const uint32_t cnt = min(chunk, n_bytes - base);
         __syncthreads();                                           // the previous chunk's masks have been consumed
         for (uint32_t j = tid; j < cnt; j += WITNESS_THREADS) {
             const Fr v = Fr::load(w + 32ull * bytes[base + j]);
@@ -212,7 +216,30 @@ __device__ void regex_coop(const DevProgram& P, uint8_t* w, uint32_t aux_off, un
             staged[j] = is_byte ? (uint8_t)v.v[0] : (uint8_t)255;  // anything else fires no transition (and fails its range checks)
         }
         __syncthreads();
-        if (tid == 0) {
+        if (tid == 0 && wide) {
+            unsigned long long live[4];
+#pragma unroll
+            for (int q = 0; q < 4; ++q)
+                live[q] = base == 0 ? (unsigned long long)ax[3 + 2 * q] | ((unsigned long long)ax[4 + 2 * q] << 32) : Q[SHA_Q_WORDS - 4 + q];
+            for (uint32_t j = 0; j < cnt; ++j) {
+                const uint32_t c = staged[j];
+                unsigned long long next[4] = {1ull, 0ull, 0ull, 0ull};
+#pragma unroll
+                for (int q = 0; q < 4; ++q) {
+                    unsigned long long m = live[q];
+                    while (m) {
+                        const uint32_t st = 64u * q + (uint32_t)(__ffsll((long long)m) - 1);
+                        m &= m - 1;
+                        const uint32_t d = table[st * 256u + c];
+                        if (d != 0xffu) next[d >> 6] |= 1ull << (d & 63u);
+                    }
+                }
+#pragma unroll
+                for (int q = 0; q < 4; ++q) { live[q] = next[q]; Q[4 * j + q] = next[q]; }
+            }
+#pragma unroll
+            for (int q = 0; q < 4; ++q) Q[SHA_Q_WORDS - 4 + q] = live[q];
+        } else if (tid == 0) {
             unsigned long long mask = base == 0 ? first : Q[SHA_Q_WORDS - 1];
             for (uint32_t j = 0; mode == 1 && j < cnt; ++j) {     // compact shape: one state, Q[j] = the product that fires
                 const uint32_t at = (uint32_t)mask * 256u + staged[j];
@@ -236,11 +263,12 @@ __device__ void regex_coop(const DevProgram& P, uint8_t* w, uint32_t aux_off, un
         }
         __syncthreads();
         for (uint32_t dd = tid; dd < n_desc; dd += WITNESS_THREADS) {
-            const uint32_t var = desc[2 * dd], ps = desc[2 * dd + 1];
+            const uint32_t var = desc[2 * dd], ps = desc[2 * dd + 1], s = ps & 255u;
             const uint32_t j = (ps >> 8) - 1u - base;              // position p reads message byte p - 1
             if (j < cnt) {
                 Fr o = Fr::zero();
-                o.v[0] = mode == 1 ? (uint32_t)(Q[j] == (ps & 255u)) : (uint32_t)((Q[j] >> (ps & 255u)) & 1ull);
+                if (wide) o.v[0] = (uint32_t)((Q[4 * j + (s >> 6)] >> (s & 63u)) & 1ull);
+                else o.v[0] = mode == 1 ? (uint32_t)(Q[j] == s) : (uint32_t)((Q[j] >> s) & 1ull);
                 o.store(w + 32ull * var);
             }
         }

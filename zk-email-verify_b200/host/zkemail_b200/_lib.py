@@ -43,6 +43,7 @@ def _sig(name, restype, argtypes):
 
 zke_circuit_build = _sig("zke_circuit_build", c_void_p, [c_char_p, ctypes.POINTER(c_i64), c_size_t, c_char_p, c_size_t])
 zke_circuit_free = _sig("zke_circuit_free", None, [c_void_p])
+zke_circuit_build_app = _sig("zke_circuit_build_app", c_void_p, [c_char_p, c_char_p, c_size_t])
 zke_circuit_from_r1cs = _sig("zke_circuit_from_r1cs", c_void_p, [c_void_p, c_size_t, c_char_p, c_size_t])
 zke_circuit_write_r1cs = _sig("zke_circuit_write_r1cs", c_i64, [c_void_p, c_void_p, c_size_t])
 zke_circuit_get_info = _sig("zke_circuit_get_info", c_int, [c_void_p, ctypes.POINTER(CircuitInfo)])

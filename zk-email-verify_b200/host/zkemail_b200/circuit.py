@@ -43,6 +43,21 @@ class Circuit:
         return cls("Regex", (msg_len,), _handle=h)
 
     @classmethod
+    def from_spec(cls, spec):
+        """An email app circuit from its spec (a dict or its JSON text; layout in app.py and at zke_circuit_build_app):
+        EmailVerifier with its flags, then the app's regexes with their revealed parts, external public inputs and an
+        optional email nullifier.  Witnesses and proofs run on the GPU like any template circuit."""
+        import json
+        text = spec if isinstance(spec, str) else json.dumps(spec)
+        err = ctypes.create_string_buffer(L.ERRCAP)
+        h = L.zke_circuit_build_app(text.encode(), err, L.ERRCAP)
+        if not h:
+            raise L.ZkeError(err.value.decode())
+        c = cls("EmailApp", (), _handle=h)
+        c.spec = json.loads(text)
+        return c
+
+    @classmethod
     def from_r1cs(cls, src):
         """circom's constraint system: an iden3 `.r1cs` (bytes, a buffer or a path, which is memory-mapped), as `circom
         --r1cs` writes it for `snarkjs groth16 setup`.  The circuit has no witness program: its witnesses come from circom's

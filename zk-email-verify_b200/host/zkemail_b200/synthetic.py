@@ -79,13 +79,13 @@ def synthetic_body(index: int, length: int = 1024, marker: str | None = None) ->
 
 
 def make_signed_email(index: int, key, body_len: int = 1024, domain: str = "example.com", selector: str = "sel",
-                      marker: str | None = None, body_override: bytes | None = None) -> bytes:
+                      marker: str | None = None, body_override: bytes | None = None, subject: str | None = None) -> bytes:
     body = body_override if body_override is not None else synthetic_body(index, body_len, marker)
     headers = [
         b"from: sender%04d@%s" % (index, domain.encode()),
         b"Content-Type: text/plain; charset=us-ascii",
         b"Mime-Version: 1.0 (Synthetic %d)" % index,
-        b"Subject: synthetic email %d" % index,
+        b"Subject: " + (subject.encode() if subject is not None else b"synthetic email %d" % index),
         b"Message-Id: <%08x@%s>" % (SEED_BASE + index, domain.encode()),
         b"Date: Sat, 14 Oct 2023 22:09:12 +0300",
         b"to: rcpt%04d@%s" % (index, domain.encode()),

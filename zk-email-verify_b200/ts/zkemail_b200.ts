@@ -5,6 +5,7 @@ import koffi from 'koffi';
 
 const lib = koffi.load(process.env.ZKEMAIL_B200_LIB ?? 'libzkemail_b200.so');
 const zke_circuit_build = lib.func('void* zke_circuit_build(const char*, const int64_t*, size_t, char*, size_t)');
+const zke_circuit_build_app = lib.func('void* zke_circuit_build_app(const char*, char*, size_t)');   // app circuit from a JSON spec
 const zke_setup = lib.func('void* zke_setup(void*, uint64_t, int, char*, size_t)');
 const zke_zkey_load = lib.func('void* zke_zkey_load(const void*, size_t, int, char*, size_t)');
 const zke_zkey_load_chunks = lib.func('void* zke_zkey_load_chunks(const void**, const size_t*, size_t, int, char*, size_t)');
@@ -28,6 +29,20 @@ const registry = new Map<string, Entry>();
 export function registerEmailVerifier(circuitName: string, params: number[], zkeyChunks: Buffer[], device = 0): void {
   const err = Buffer.alloc(4096);
   const circuit = zke_circuit_build('EmailVerifier', BigInt64Array.from(params.map(BigInt)), params.length, err, err.length);
+  if (!circuit) throw new Error(cstr(err));
+  const zkey = zkeyChunks.length === 1
+    ? zke_zkey_load(zkeyChunks[0], zkeyChunks[0].length, device, err, err.length)
+    : zke_zkey_load_chunks(zkeyChunks, BigUint64Array.from(zkeyChunks.map((c) => BigInt(c.length))), zkeyChunks.length, device, err, err.length);
+  if (!zkey) throw new Error(cstr(err));
+  const ctx = zke_ctx_open(circuit, zkey, device, 1, err, err.length);
+  if (!ctx) throw new Error(cstr(err));
+  registry.set(circuitName, { circuit, zkey, ctx });
+}
+
+/** registerEmailVerifier for an app circuit built from its spec (Circuit.from_spec in Python; layout at zke_circuit_build_app). */
+export function registerEmailApp(circuitName: string, spec: object | string, zkeyChunks: Buffer[], device = 0): void {
+  const err = Buffer.alloc(4096);
+  const circuit = zke_circuit_build_app(typeof spec === 'string' ? spec : JSON.stringify(spec), err, err.length);
   if (!circuit) throw new Error(cstr(err));
   const zkey = zkeyChunks.length === 1
     ? zke_zkey_load(zkeyChunks[0], zkeyChunks[0].length, device, err, err.length)
