@@ -359,6 +359,30 @@ void zke_verifier_close(zke_verifier* v);
  * Returns the number of valid proofs, < 0 on a fatal error. */
 int zke_verifier_batch(zke_verifier* v, size_t n, const uint8_t* proofs, const uint8_t* publics, const uint8_t* rand16,
                        uint8_t* ok, char* err, size_t errcap);
+/* ---- Proof aggregation (SnarkPack; DESIGN.md "Proof aggregation") -------------------------------------------------
+ * n Groth16 proofs under one key (n a power of two from 2 to 8192) -> one proof of zke_agg_bytes(n) = 3008 + 3968 log2 n
+ * bytes that the host checks with O(log n) pairings.  The SRS holds the powers of two independent taus a and b, read
+ * from the tauG1 / tauG2 sections of two `.ptau` files of power >= log2(n_max) + 1 (prepared or not; points checked on
+ * GPU `device`; both must start from the same generators). */
+typedef struct zke_agg_srs zke_agg_srs;
+zke_agg_srs* zke_agg_srs_from_ptau(const void* ptau_a, size_t len_a, const void* ptau_b, size_t len_b, uint32_t n_max, int device,
+                                   char* err, size_t errcap);
+void zke_agg_srs_free(zke_agg_srs* s);
+uint32_t zke_agg_srs_n_max(const zke_agg_srs* s);
+/* The verifier key {"protocol":"snarkpack", g, h, g_a, g_b, h_a, h_b} (snarkjs point encoding); *len in/out as
+ * zke_zkey_vkey_json (-2: buffer too small, *len = bytes needed). */
+int zke_agg_vk_json(const zke_agg_srs* s, char* out, size_t* len);
+/* Bytes of an aggregate of n proofs; 0 for an n that cannot be aggregated. */
+size_t zke_agg_bytes(size_t n);
+/* proofs: [n][8][32] and publics: [n][n_public][32] in zke_prove's layout; vkey_json: snarkjs vkey.json.  Writes
+ * zke_agg_bytes(n) bytes to `out` and returns that count, < 0 on a refusal (n, SRS size, a proof point off its curve or
+ * outside its subgroup, a public signal not below r) with the reason in err. */
+int64_t zke_aggregate(zke_agg_srs* s, const char* vkey_json, size_t n, const uint8_t* proofs, const uint8_t* publics, uint8_t* out,
+                      size_t cap, char* err, size_t errcap);
+/* Host only: 1 if `agg` proves n valid proofs under vkey_json for these public signals ([n][n_public][32]), 0 if not,
+ * < 0 on malformed input (n, lengths, unreduced coordinates, points off their curves or outside their subgroups). */
+int zke_agg_verify(const char* agg_vk_json, const char* vkey_json, size_t n, const uint8_t* publics, const uint8_t* agg, size_t agg_len,
+                   char* err, size_t errcap);
 /* Diagnostic: e(P_i, Q_i) for n pairs on GPU `device`, in zke_pairing_alphabeta's output layout (g1: [n][64],
  * g2: [n][128], out: [n][384]; standard form LE).  Points must be on their curves (< 0 otherwise). */
 int zke_selftest_pairing_gpu(int device, size_t n, const uint8_t* g1, const uint8_t* g2, uint8_t* out, char* err, size_t errcap);

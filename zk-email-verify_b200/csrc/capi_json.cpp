@@ -8,6 +8,7 @@
 #include "engine.hpp"
 #include "ec_host.hpp"
 #include "gadgets.hpp"
+#include "aggregate_host.hpp"
 #include <cstring>
 #include <memory>
 #include <random>
@@ -294,6 +295,21 @@ VerifyingKey zke::vkey_from_json(const char* json) {
     for (auto& p : need(vk, "IC").arr) k.ic.push_back(g1_of(p));
     if (k.ic.empty()) throw std::runtime_error("vkey has no IC");
     return k;
+}
+
+agg::AggVk zke::agg::agg_vk_from_json(const char* json) {
+    JV o = JParser(json).parse();
+    const JV* prot = o.get("protocol");
+    if (!prot || prot->s != "snarkpack") throw std::runtime_error("aggregation key protocol is not snarkpack");
+    AggVk k;
+    k.g = g1_of(need(o, "g")); k.g_a = g1_of(need(o, "g_a")); k.g_b = g1_of(need(o, "g_b"));
+    k.h = g2_of(need(o, "h")); k.h_a = g2_of(need(o, "h_a")); k.h_b = g2_of(need(o, "h_b"));
+    return k;
+}
+
+std::string zke::agg::agg_vk_to_json(const AggVk& k) {
+    return "{\"protocol\":\"snarkpack\",\"curve\":\"bn128\",\"g\":" + g1_json(k.g) + ",\"h\":" + g2_json(k.h) +
+           ",\"g_a\":" + g1_json(k.g_a) + ",\"g_b\":" + g1_json(k.g_b) + ",\"h_a\":" + g2_json(k.h_a) + ",\"h_b\":" + g2_json(k.h_b) + "}";
 }
 
 extern "C" {

@@ -1542,3 +1542,4 @@ int zke_shard_combine_raw(const uint8_t* key_points, const uint8_t* partials, in
 // because it builds zke_zkey objects the same way do_setup / do_zkey_load do.
 #include "setup.cu"
 #include "ptau.cu"
+#include "aggregate.cu"

@@ -765,7 +765,8 @@ size_t MsmPlan<F>::workspace_bytes(uint32_t n, const MsmConfig& cfg) {
     al(sizeof(XYZZ<F>) * (max_chunks / PASS_FANIN + n_buckets + 1));  // partial (ping-pong for the extra passes)
     al(4 * (n_buckets + 1));           // second offsets array
     al(sizeof(XYZZ<F>) * groups);      // group sums
-    al(sizeof(XYZZ<F>) * ((size_t)n / LIST_FANIN + 2) * 2);  // list reduction ping-pong
+    al(sizeof(XYZZ<F>) * ((size_t)n / LIST_FANIN + 2));      // list reduction ping-pong: two arrays, each padded as run() takes it
+    al(sizeof(XYZZ<F>) * ((size_t)n / LIST_FANIN + 2));
     if (cfg.ba_levels > 0 && sizeof(F) == 32) al(BaPlan<F>::bytes(max_entries, n_buckets, cfg.ba_levels));
     const size_t order_cells = ((max_chunks + ORDER_BLOCK - 1) / ORDER_BLOCK) * cfg.chunk;
     al(4 * max_chunks);                       // order

@@ -12,7 +12,8 @@
 // ffjavascript / wasmcurves use, so final_exponentiation(miller_loop(Q, P)) is the reduced pairing raised to
 // 2 z (6 z^2 + 3 z + 1), z = 4965661367192848881 - the value zke_pairing_alphabeta returns.
 //
-// Compiles under ZKE_FF_EMULATE with g++ like ec.cuh (tests/test_pairing_emulation.py).
+// Compiles under ZKE_FF_EMULATE with g++ like ec.cuh (tests/test_pairing_emulation.py).  verify.cu and engine.cu
+// (aggregate.cu) both include it: the out-of-line functions are `inline` for the linkage.
 #pragma once
 #include "ec.cuh"
 #include <cstddef>
@@ -193,7 +194,7 @@ struct G2Proj { Fq2 x, y, z; };   // homogeneous projective: x = X/Z, y = Y/Z
 // R <- 2R; tangent at R (Costello-Lange-Naehrig, as in arkworks' BN doubling step), coordinates scaled by 4 to avoid halving:
 // X' = 2 XY (B - F), Y' = (B + F)^2 - 12 E^2, Z' = 4 B H with B = Y^2, E = 3 b' Z^2, F = 3E, H = 2YZ;
 // line = (-H, 3 X^2, E - B)
-__device__ __noinline__ LineCoeffs dbl_step(G2Proj& r) {
+inline __device__ __noinline__ LineCoeffs dbl_step(G2Proj& r) {
     const Fq2 B = r.y.sqr(), C = r.z.sqr();
     const Fq2 E = fq2_from(TWIST_B) * (C.dbl() + C);
     const Fq2 F = E.dbl() + E;
@@ -209,7 +210,7 @@ __device__ __noinline__ LineCoeffs dbl_step(G2Proj& r) {
     return l;
 }
 // R <- R + Q (Q affine); chord through R and Q: theta = Y - qy Z, lambda = X - qx Z; line = (lambda, -theta, theta qx - lambda qy)
-__device__ __noinline__ LineCoeffs add_step(G2Proj& r, const G2Affine& q) {
+inline __device__ __noinline__ LineCoeffs add_step(G2Proj& r, const G2Affine& q) {
     const Fq2 theta = r.y - q.y * r.z, lambda = r.x - q.x * r.z;
     const Fq2 C = theta.sqr(), D = lambda.sqr();
     const Fq2 E = lambda * D, F = r.z * C, G = r.x * D;
@@ -274,7 +275,7 @@ __device__ Fq12 miller_loop(bool fly, const G2Affine& q, const G1Affine& p, cons
 
 // ---- final exponentiation -------------------------------------------------------------------------------------------
 // x^(-z) on the cyclotomic subgroup
-__device__ Fq12 cyclotomic_exp_neg_z(const Fq12& x) {
+inline __device__ Fq12 cyclotomic_exp_neg_z(const Fq12& x) {
     Fq12 r = x;
     for (int i = 61; i >= 0; --i) {     // bit 62 is the top bit of z
         r = r.cyclotomic_sqr();
@@ -283,7 +284,7 @@ __device__ Fq12 cyclotomic_exp_neg_z(const Fq12& x) {
     return r.conj();
 }
 // f^((p^12 - 1) / r) raised to 2 z (6 z^2 + 3 z + 1): easy part f^((p^6 - 1)(p^2 + 1)), then the Fuentes-Castaneda hard part
-__device__ Fq12 final_exponentiation(const Fq12& f) {
+inline __device__ Fq12 final_exponentiation(const Fq12& f) {
     Fq12 m = f.conj() * f.inv();
     m = m.frobenius<2>() * m;
     const Fq12 y0 = cyclotomic_exp_neg_z(m);

@@ -6,7 +6,9 @@
 // polynomials (w^6 = 9 + u), point arithmetic on the sextic twist in Fq2 (affine), line functions embedded as
 // sparse Fq12 elements, final exponentiation by plain square-and-multiply with the exponent (p^12 - 1)/r.
 #include "ec_host.hpp"
+#include "aggregate_host.hpp"
 #include <array>
+#include <cstring>
 
 namespace zke {
 
@@ -203,6 +205,41 @@ void pairing_alphabeta(const G1AffineH& alpha1, const G2AffineH& beta2, U256 out
             out[(i * 3 + j) * 2 + 1] = e.c[n + 6].to_u256();
         }
 }
+
+// GT arithmetic for the aggregate verifier (aggregate_host.hpp): values normalised like pairing_alphabeta
+namespace agg {
+Gt gt_one() { return Gt{F12::one().c}; }
+Gt gt_mul(const Gt& a, const Gt& b) { return Gt{mul(F12{a.c}, F12{b.c}).c}; }
+Gt gt_pow(const Gt& a, const U256& e) { return Gt{pow_u256(F12{a.c}, e).c}; }
+Gt gt_pairing_product(const std::vector<std::pair<G1AffineH, G2AffineH>>& terms) {
+    static const U256 K = u256_from_hex("3bec47df15e307c81ea96b02d9d9e38d2e5d4e223ddedaf4");
+    F12 f = F12::one();
+    for (auto& t : terms) f = mul(f, miller_loop(t.second, t.first));
+    return Gt{pow_u256(final_exponentiation(f), K).c};
+}
+void gt_store(const Gt& e, uint8_t out[384]) {
+    const Fq nine = Fq::from_u64(9);
+    for (int i = 0; i < 2; ++i)
+        for (int j = 0; j < 3; ++j) {
+            const int n = 2 * j + i;
+            const U256 a = (e.c[n] + nine * e.c[n + 6]).to_u256(), b = e.c[n + 6].to_u256();
+            memcpy(out + 64 * (3 * i + j), a.v, 32);
+            memcpy(out + 64 * (3 * i + j) + 32, b.v, 32);
+        }
+}
+Gt gt_load(const uint8_t* in) {
+    const Fq nine = Fq::from_u64(9);
+    Gt e;
+    for (int i = 0; i < 2; ++i)
+        for (int j = 0; j < 3; ++j) {
+            const int n = 2 * j + i;
+            const Fq a = fq_at(in + 64 * (3 * i + j)), b = fq_at(in + 64 * (3 * i + j) + 32);
+            e.c[n] = a - nine * b;
+            e.c[n + 6] = b;
+        }
+    return e;
+}
+}  // namespace agg
 
 bool pairing_product_is_one(const std::vector<std::pair<G1AffineH, G2AffineH>>& terms) {
     F12 f = F12::one();

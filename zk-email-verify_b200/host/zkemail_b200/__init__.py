@@ -13,6 +13,7 @@ from .app import decode_app_outputs, generate_app_inputs  # noqa: F401
 from .engine import AssertFailed, Context, Verifier, Zkey, device_count, proof_to_json, verify, verify_batch  # noqa: F401
 from .engine import ptau_info, ptau_toy, verify_zkey  # noqa: F401
 from .engine import ptau_contribute, ptau_new, ptau_prepare, ptau_report, verify_ptau  # noqa: F401
+from .aggregate import AggSrs, aggregate, verify_aggregate  # noqa: F401
 from .chunked_zkey import (generate_proof, verify_proof, register_circuit, register_zkey_files, generateProof, verifyProof,  # noqa: F401
                            InsecureKeyError)
 from . import synthetic  # noqa: F401,E402

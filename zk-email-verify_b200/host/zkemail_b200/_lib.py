@@ -121,6 +121,13 @@ zke_ptau_contribute = _sig("zke_ptau_contribute", c_i64, [c_void_p, c_size_t, c_
 zke_ptau_prepare = _sig("zke_ptau_prepare", c_i64, [c_void_p, c_size_t, c_int, c_void_p, c_size_t, c_char_p, c_size_t])
 zke_ptau_prepare_timing = _sig("zke_ptau_prepare_timing", c_int, [ctypes.POINTER(ctypes.c_double), ctypes.POINTER(ctypes.c_double)])
 zke_ptau_verify = _sig("zke_ptau_verify", c_int, [c_void_p, c_size_t, c_void_p, c_size_t, c_void_p, c_void_p, c_int, c_char_p, c_size_t])
+zke_agg_srs_from_ptau = _sig("zke_agg_srs_from_ptau", c_void_p, [c_void_p, c_size_t, c_void_p, c_size_t, c_u32, c_int, c_char_p, c_size_t])
+zke_agg_srs_free = _sig("zke_agg_srs_free", None, [c_void_p])
+zke_agg_srs_n_max = _sig("zke_agg_srs_n_max", c_u32, [c_void_p])
+zke_agg_vk_json = _sig("zke_agg_vk_json", c_int, [c_void_p, c_char_p, ctypes.POINTER(c_size_t)])
+zke_agg_bytes = _sig("zke_agg_bytes", c_size_t, [c_size_t])
+zke_aggregate = _sig("zke_aggregate", c_i64, [c_void_p, c_char_p, c_size_t, c_void_p, c_void_p, c_void_p, c_size_t, c_char_p, c_size_t])
+zke_agg_verify = _sig("zke_agg_verify", c_int, [c_char_p, c_char_p, c_size_t, c_void_p, c_void_p, c_size_t, c_char_p, c_size_t])
 zke_selftest_fpmul_hint =_sig("zke_selftest_fpmul_hint", c_int, [c_u32, c_u32, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p])
 
 (SEC_ALPHA1, SEC_BETA1, SEC_DELTA1, SEC_BETA2, SEC_GAMMA2, SEC_DELTA2) = (101, 102, 103, 104, 105, 106)

@@ -16,6 +16,12 @@ const zke_fullprove_json = lib.func('int zke_fullprove_json(void*, void*, const 
 const zke_verify_json = lib.func('int zke_verify_json(const char*, const char*, const char*, char*, size_t)');
 const zke_verify_batch_json = lib.func('int zke_verify_batch_json(const char*, const char*, const char*, const uint8_t*, uint8_t*, char*, size_t)');
 
+const zke_agg_srs_from_ptau = lib.func('void* zke_agg_srs_from_ptau(const void*, size_t, const void*, size_t, uint32_t, int, char*, size_t)');
+const zke_agg_vk_json = lib.func('int zke_agg_vk_json(void*, char*, size_t*)');
+const zke_agg_bytes = lib.func('size_t zke_agg_bytes(size_t)');
+const zke_aggregate = lib.func('int64_t zke_aggregate(void*, const char*, size_t, const uint8_t*, const uint8_t*, uint8_t*, size_t, char*, size_t)');
+const zke_agg_verify = lib.func('int zke_agg_verify(const char*, const char*, size_t, const uint8_t*, const uint8_t*, size_t, char*, size_t)');
+
 const cstr = (b: Buffer) => b.toString('utf8', 0, b.indexOf(0));
 type Entry = { circuit: unknown; zkey: unknown; ctx: unknown };
 const registry = new Map<string, Entry>();
@@ -99,5 +105,30 @@ export const groth16 = {
     const rc = zke_verify_batch_json(JSON.stringify(vkey), JSON.stringify(publicSignals), JSON.stringify(proofs), rand, ok, err, err.length);
     if (rc < 0) throw new Error(cstr(err));
     return Array.from(ok).map((b) => b === 1);
+  },
+};
+
+/** Proof aggregation (SnarkPack, not in snarkjs): n proofs under one key -> one O(log n) proof.  `proofs` / `publics` are
+ * zke_prove's binary layouts ([n][8][32], [n][nPublic][32]); the SRS comes from two `.ptau` files with independent taus. */
+export const aggregation = {
+  srsFromPtau(ptauA: Buffer, ptauB: Buffer, nMax: number, device = 0): { srs: unknown; vk: object } {
+    const err = Buffer.alloc(4096);
+    const srs = zke_agg_srs_from_ptau(ptauA, ptauA.length, ptauB, ptauB.length, nMax, device, err, err.length);
+    if (!srs) throw new Error(cstr(err));
+    const buf = Buffer.alloc(4096), len = [buf.length];
+    if (zke_agg_vk_json(srs, buf, len) !== 0) throw new Error('zke_agg_vk_json failed');
+    return { srs, vk: JSON.parse(cstr(buf)) };
+  },
+  aggregate(srs: unknown, vkey: object, n: number, proofs: Buffer, publics: Buffer): Buffer {
+    const out = Buffer.alloc(Number(zke_agg_bytes(n)) || 1), err = Buffer.alloc(4096);
+    const rc = zke_aggregate(srs, JSON.stringify(vkey), n, proofs, publics, out, out.length, err, err.length);
+    if (rc < 0) throw new Error(cstr(err));
+    return out.subarray(0, Number(rc));
+  },
+  verify(aggVk: object, vkey: object, n: number, publics: Buffer, agg: Buffer): boolean {
+    const err = Buffer.alloc(4096);
+    const rc = zke_agg_verify(JSON.stringify(aggVk), JSON.stringify(vkey), n, publics, agg, agg.length, err, err.length);
+    if (rc < 0) throw new Error(cstr(err));
+    return rc === 1;
   },
 };
