@@ -109,12 +109,17 @@ enum {
     ZKE_ARR_SHA_BLOCKS = 17, /* uint32: {n_blocks, per block: var_begin, var_end, temp_begin, temp_end, n_desc,
                                inputs[768], desc[n_desc][2] = {signal, quantity << 8 | bit}} - the Sha256compression
                                instances the engine evaluates natively (one compression instead of ~320 levels)  */
-    ZKE_ARR_REGEX_SEEDS = 18 /* uint32: {n_seeds, per seed: n_desc, n_bytes, n_states | wide << 30 | mode << 31,
+    ZKE_ARR_REGEX_SEEDS = 18,/* uint32: {n_seeds, per seed: n_desc, n_bytes, n_states | wide << 30 | mode << 31,
                                first_mask lo, hi (wide = zk-regex shape with 65..255 states: 8 words, the 256-bit live set
                                from its low word up), bytes[n_bytes] (signal of message byte j), table[n_states * 64] (destination state of
                                (source, byte), 0xff = none, 4 per word), mode 1 (compact shape): group[n_states * 64] (the
                                product that fires), desc[n_desc][2] = {signal, position << 8 | state or product}} - the
                                regex instances whose chained signals the engine seeds with one automaton run      */
+    ZKE_ARR_POSEIDON_BLOCKS = 19 /* uint32: {n_blocks, per block: t, var_begin, var_end, temp_begin, temp_end, n_desc,
+                               inputs[t - 1], desc[n_desc][2] = {signal, round << 16 | lane << 8 | kind}}, kind 0 input copy,
+                               1 x^2, 2 x^4, 3 x^5 (the S-box of round `round`), 4 mix output of round `round` - the Poseidon
+                               instances of hashed and committed app outputs, which the engine evaluates natively (one
+                               permutation instead of ~4 levels per round)                                          */
 };
 const void* zke_circuit_array(const zke_circuit* c, int which, size_t* n_elems);
 const char* zke_circuit_scope_name(const zke_circuit* c, uint32_t scope_index);
@@ -122,7 +127,7 @@ const char* zke_circuit_scope_name(const zke_circuit* c, uint32_t scope_index);
 /* What the engine's lowering of the witness program builds for this circuit (the stream the witness kernel walks: the native
  * SHA-256 and regex-seeding substitutions, levels cut into iterations of 512 records and padded to rounds of `cluster`
  * iterations), computed on the host - no device needed.  zke_ctx_open lowers with the same code; its options come from
- * ZKE_NATIVE_SHA, ZKE_NATIVE_REGEX, ZKE_COOP_FPMUL (default 1 each) and ZKE_WITNESS_CLUSTER (default: chosen from max_batch).
+ * ZKE_NATIVE_SHA, ZKE_NATIVE_REGEX, ZKE_COOP_FPMUL, ZKE_NATIVE_POSEIDON (default 1 each) and ZKE_WITNESS_CLUSTER (default: chosen from max_batch).
  * cluster: 1, 2, 4 or 8.  level_ops (optional, may be NULL): the first min(n_levels, level_cap) entries receive the number of
  * records of each level that are not cooperative ops.  A circuit read from an `.r1cs` has no program: an error.
  * Returns 0, or non-zero with a message in err. */
@@ -139,6 +144,19 @@ typedef struct zke_program_stats {
 } zke_program_stats;
 int zke_circuit_program_stats(const zke_circuit* c, int native_sha, int native_regex, int coop_fpmul, uint32_t cluster,
                               zke_program_stats* out, uint32_t* level_ops, size_t level_cap, char* err, size_t errcap);
+/* The same with every lowering option as a flag (zke_circuit_program_stats lowers with native Poseidon on).  The engine's
+ * native Poseidon follows ZKE_NATIVE_POSEIDON (default 1). */
+enum {
+    ZKE_LOWER_NATIVE_SHA = 1, ZKE_LOWER_NATIVE_REGEX = 2, ZKE_LOWER_COOP_FPMUL = 4, ZKE_LOWER_NATIVE_POSEIDON = 8,
+    ZKE_LOWER_ALL = 15
+};
+int zke_circuit_program_stats_ex(const zke_circuit* c, uint32_t flags, uint32_t cluster, zke_program_stats* out,
+                                 uint32_t* level_ops, size_t level_cap, char* err, size_t errcap);
+
+/* Poseidon(n) of n = 1..16 field elements (32-byte little-endian, each below r) into out[32]: circomlib's parameters, the
+ * permutation the circuits constrain (the `poseidon` of @zk-email/helpers).  Returns 0, -1 for a bad n or pointer, -2 for an
+ * input not below r. */
+int zke_poseidon_hash(const uint8_t* inputs, size_t n, uint8_t* out);
 
 
 /* ---------------------------------------------------------------------------------------------------

@@ -353,6 +353,7 @@ const void* zke_circuit_array(const zke_circuit* c, int which, size_t* n) {
         case ZKE_ARR_SCOPE_OF_CONSTRAINT: RET(k.scope_of_constraint);
         case ZKE_ARR_SHA_BLOCKS: RET(k.sha_flat);
         case ZKE_ARR_REGEX_SEEDS: RET(k.regex_flat);
+        case ZKE_ARR_POSEIDON_BLOCKS: RET(k.poseidon_flat);
         default: *n = 0; return nullptr;
     }
 #undef RET
@@ -365,12 +366,22 @@ const char* zke_circuit_scope_name(const zke_circuit* c, uint32_t i) {
 
 int zke_circuit_program_stats(const zke_circuit* c, int native_sha, int native_regex, int coop_fpmul, uint32_t cluster,
                               zke_program_stats* out, uint32_t* level_ops, size_t level_cap, char* err, size_t errcap) {
+    const uint32_t flags = (native_sha ? ZKE_LOWER_NATIVE_SHA : 0u) | (native_regex ? ZKE_LOWER_NATIVE_REGEX : 0u) |
+                           (coop_fpmul ? ZKE_LOWER_COOP_FPMUL : 0u) | ZKE_LOWER_NATIVE_POSEIDON;
+    return zke_circuit_program_stats_ex(c, flags, cluster, out, level_ops, level_cap, err, errcap);
+}
+
+int zke_circuit_program_stats_ex(const zke_circuit* c, uint32_t flags, uint32_t cluster, zke_program_stats* out,
+                                 uint32_t* level_ops, size_t level_cap, char* err, size_t errcap) {
     try {
         if (!c || !out) throw std::runtime_error("null argument");
         if (c->c.r1cs_only) throw std::runtime_error(R1CS_NO_PROGRAM);
         if (cluster != 1 && cluster != 2 && cluster != 4 && cluster != 8) throw std::runtime_error("cluster must be 1, 2, 4 or 8");
+        if (flags & ~(uint32_t)ZKE_LOWER_ALL) throw std::runtime_error("unknown lowering flag");
         LowerOptions opt;
-        opt.native_sha = native_sha != 0; opt.native_regex = native_regex != 0; opt.coop_fpmul = coop_fpmul != 0; opt.cluster = cluster;
+        opt.native_sha = (flags & ZKE_LOWER_NATIVE_SHA) != 0; opt.native_regex = (flags & ZKE_LOWER_NATIVE_REGEX) != 0;
+        opt.coop_fpmul = (flags & ZKE_LOWER_COOP_FPMUL) != 0; opt.native_poseidon = (flags & ZKE_LOWER_NATIVE_POSEIDON) != 0;
+        opt.cluster = cluster;
         const WitnessStream S = lower_witness_program(c->c, coef_words(c->c.coefs), opt);
         memset(out, 0, sizeof *out);
         out->n_levels = S.n_levels; out->n_iters = S.n_iters; out->cluster = S.cluster;
@@ -389,6 +400,20 @@ int zke_circuit_program_stats(const zke_circuit* c, int native_sha, int native_r
         set_err(err, errcap, e.what());
         return -1;
     }
+}
+
+int zke_poseidon_hash(const uint8_t* inputs, size_t n, uint8_t* out) {
+    if (!inputs || !out || n < 1 || n > 16) return -1;
+    std::vector<Fr> in(n);
+    for (size_t i = 0; i < n; ++i) {
+        U256 x;
+        memcpy(x.v, inputs + 32 * i, 32);
+        if (u256_cmp(x, fr_params().p) >= 0) return -2;
+        in[i] = Fr::from_u256(x);
+    }
+    const U256 h = gadgets::poseidon_hash(in).to_u256();
+    memcpy(out, h.v, 32);
+    return 0;
 }
 
 int zke_selftest_fpmul_hint(uint32_t n, uint32_t k, const uint8_t* a, const uint8_t* b, const uint8_t* p, uint8_t* q, uint8_t* r) {

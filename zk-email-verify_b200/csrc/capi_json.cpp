@@ -253,11 +253,23 @@ gadgets::AppSpec app_spec_of(const JV& s) {
             for (size_t i = 0; i < parts->arr.size(); ++i) {
                 const JV& pt = parts->arr[i];
                 const std::string pf = f + "parts[" + std::to_string(i) + "]";
-                only_keys(pt, pf, {"regexDef", "isPublic", "maxLength"});
+                only_keys(pt, pf, {"regexDef", "isPublic", "maxLength", "reveal", "salt"});
                 gadgets::AppRegexPart part;
                 part.regex = str_of(pt, "regexDef", pf + ".");
                 part.is_public = bool_of(pt, "isPublic", false, pf + ".");
                 if (const JV* ml = pt.get("maxLength")) part.max_length = uint_of(*ml, pf + ".maxLength");
+                if (pt.get("reveal")) {
+                    const std::string rv = str_of(pt, "reveal", pf + ".");
+                    if (rv == "bytes") part.reveal = gadgets::REVEAL_BYTES;
+                    else if (rv == "hash") part.reveal = gadgets::REVEAL_HASH;
+                    else if (rv == "commit") part.reveal = gadgets::REVEAL_COMMIT;
+                    else throw std::runtime_error(pf + ".reveal: '" + rv + "' is none of \"bytes\", \"hash\", \"commit\"");
+                    part.reveal_given = true;
+                }
+                if (pt.get("salt")) {
+                    part.salt = str_of(pt, "salt", pf + ".");
+                    if (part.salt.empty()) throw std::runtime_error(pf + ".salt: empty name");
+                }
                 rx.parts.push_back(part);
             }
             a.regexes.push_back(rx);
@@ -266,9 +278,10 @@ gadgets::AppSpec app_spec_of(const JV& s) {
     if (const JV* es = array_of(s, "externalInputs")) {
         for (size_t i = 0; i < es->arr.size(); ++i) {
             const std::string f = "externalInputs[" + std::to_string(i) + "]";
-            only_keys(es->arr[i], f, {"name", "maxLength"});
+            only_keys(es->arr[i], f, {"name", "maxLength", "isPublic"});
             gadgets::AppExternalInput ei;
             ei.name = str_of(es->arr[i], "name", f + ".");
+            ei.is_public = bool_of(es->arr[i], "isPublic", true, f + ".");
             if (const JV* ml = es->arr[i].get("maxLength")) {
                 ei.max_length = uint_of(*ml, f + ".maxLength");
                 if (ei.max_length == 0) throw std::runtime_error(f + ".maxLength: must be positive (leave it out for one field element)");

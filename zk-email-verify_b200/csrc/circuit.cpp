@@ -288,6 +288,15 @@ Circuit Builder::finalize() {
         append_regex_seed(c.regex_flat, R);
     }
 
+    for (auto& blk : c.poseidon_blocks) { blk.temp_begin += m; blk.temp_end += m; }
+    c.poseidon_flat.clear();
+    c.poseidon_flat.push_back((uint32_t)c.poseidon_blocks.size());
+    for (auto& blk : c.poseidon_blocks) {
+        c.poseidon_flat.insert(c.poseidon_flat.end(), {blk.t, blk.var_begin, blk.var_end, blk.temp_begin, blk.temp_end, (uint32_t)(blk.desc.size() / 2)});
+        c.poseidon_flat.insert(c.poseidon_flat.end(), blk.inputs.begin(), blk.inputs.end());
+        c.poseidon_flat.insert(c.poseidon_flat.end(), blk.desc.begin(), blk.desc.end());
+    }
+
     // Fuse "scratch <- LC; bits <- (scratch >> k) & mask" into OP_SHRLC when the scratch slot feeds nothing else:
     // the shift ops then sit one dependency level earlier (13.9 k -> 10.8 k levels for the default EmailVerifier).
     // ZKE_FUSED_SHRAND=0 keeps the two-op form (GPU witness == oracle verified in both forms).

@@ -115,6 +115,22 @@ struct RegexSeed {
 
 void append_regex_seed(std::vector<uint32_t>& out, const RegexSeed& R);   // flat image (circuit.cpp)
 
+// One Poseidon(t - 1) instance as the front end built it (poseidon.cpp: poseidon with a record): every signal the gadget
+// creates is a lane of the permutation's state at some round - the copy of an input, x^2, x^4 or x^5 of the S-box, or the
+// output of the mix - so a device can produce all of them from ONE native permutation instead of walking the gadget's
+// ~4 dependency levels per round.  As for ShaBlock, the witness program keeps all of its ops (the CPU oracle walks them);
+// the record only lets the engine substitute the sub-program (witness_program.cpp).
+struct PoseidonBlock {
+    uint32_t t = 0;                           // width: t - 1 inputs, state lane 0 starts at zero
+    std::vector<uint32_t> inputs;             // t - 1 variables
+    uint32_t var_begin = 0, var_end = 0;      // signals created by the gadget: [var_begin, var_end), one descriptor each
+    uint32_t temp_begin = 0, temp_end = 0;    // scratch slots of its long mix sums (absolute slot numbers after finalize)
+    std::vector<uint32_t> desc;               // 2 words per created signal: {variable, round << 16 | lane << 8 | kind}
+};
+enum PoseidonKind : uint32_t { POS_K_INPUT = 0, POS_K_X2 = 1, POS_K_X4 = 2, POS_K_X5 = 3, POS_K_MIX = 4 };
+// (input copies carry round 0; x^k of round r is the S-box of the state after round r's constants; mix of round r is the
+// state after round r)
+
 struct SignalGroup {
     std::string name;
     uint32_t first;  // first witness index
@@ -157,6 +173,11 @@ struct Circuit {
     // lo, hi (wide: 8 words, the 256-bit mask from its low word up), bytes[n_bytes], table[n_states * 64] (4 bytes per word, little-endian), mode 1: group[n_states * 64], desc[2 n_desc]}
     // (built by finalize; ZKE_ARR_REGEX_SEEDS); the engine appends the same image to the program's aux table
     std::vector<uint32_t> regex_flat;
+
+    std::vector<PoseidonBlock> poseidon_blocks;   // Poseidon instances eligible for native evaluation (may be empty)
+    // flat image of poseidon_blocks: {n_blocks, then per block: t, var_begin, var_end, temp_begin, temp_end, n_desc,
+    // inputs[t - 1], desc[2 n_desc]} (built by finalize; ZKE_ARR_POSEIDON_BLOCKS)
+    std::vector<uint32_t> poseidon_flat;
 
     // Read from an iden3 `.r1cs` (r1cs.cpp): the constraint system alone.  The witness program above is empty, witnesses
     // come from elsewhere (circom's witness calculator); nLabels and the section-3 wire -> label map are kept so that the
@@ -214,6 +235,7 @@ class Builder {
     uint32_t num_temps() const { return next_temp_; }
     void add_sha_block(ShaBlock&& blk) { c_.sha_blocks.push_back(std::move(blk)); }   // temp range as raw temp indices
     void add_regex_seed(RegexSeed&& sd) { c_.regex_seeds.push_back(std::move(sd)); }
+    void add_poseidon_block(PoseidonBlock&& blk) { c_.poseidon_blocks.push_back(std::move(blk)); }   // temp range as raw temp indices
     uint32_t num_constraints() const { return (uint32_t)c_.scope_of_constraint.size(); }
 
    private:

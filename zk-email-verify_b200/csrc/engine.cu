@@ -560,6 +560,7 @@ static void upload_program(zke_ctx* x, const Circuit& c) {
     // ZKE_COOP_FPMUL=0: the sequential single-thread hint
     if (const char* e = getenv("ZKE_NATIVE_SHA")) opt.native_sha = atoi(e) != 0;
     if (const char* e = getenv("ZKE_NATIVE_REGEX")) opt.native_regex = atoi(e) != 0;
+    if (const char* e = getenv("ZKE_NATIVE_POSEIDON")) opt.native_poseidon = atoi(e) != 0;   // 0: the recorded Poseidon gadgets' own ops
     if (const char* e = getenv("ZKE_COOP_FPMUL")) opt.coop_fpmul = atoi(e) != 0;
     // ZKE_WITNESS_CLUSTER = 2 / 4 / 8: thread-block cluster of that many CTAs per email (witness.cu); every level is padded to
     // whole rounds of `cluster` iterations, iteration k belongs to CTA k % cluster

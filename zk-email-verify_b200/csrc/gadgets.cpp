@@ -830,15 +830,15 @@ LC poseidon_large(Builder& b, uint32_t bits_per_chunk, const LCVec& in) {
     return poseidon(b, pin);
 }
 
-LC poseidon_modular(Builder& b, const LCVec& in) {
+LC poseidon_modular(Builder& b, const LCVec& in, bool record) {
     ScopeGuard g(b, "PoseidonModular");
     const size_t n = in.size();
     if (n == 0) throw std::runtime_error("PoseidonModular: no inputs");
     LC out;
     for (size_t start = 0, i = 0; start < n; start += 16, ++i) {
         const size_t end = std::min(n, start + 16);
-        LC chunk_hash = poseidon(b, LCVec(in.begin() + start, in.begin() + end));   // Slice + Poseidon(16 | last_chunk_size)
-        out = (i == 0) ? chunk_hash : poseidon(b, {out, chunk_hash});                // _out = Poseidon(2)([_out, chunk_hash])
+        LC chunk_hash = poseidon(b, LCVec(in.begin() + start, in.begin() + end), record);   // Slice + Poseidon(16 | last_chunk_size)
+        out = (i == 0) ? chunk_hash : poseidon(b, {out, chunk_hash}, record);                // _out = Poseidon(2)([_out, chunk_hash])
     }
     return out;
 }
@@ -928,7 +928,7 @@ Circuit build_email_app(const AppSpec& A, bool materialize_linear) {
             if (t == name) throw std::runtime_error(field + ": signal name '" + name + "' is used twice");
         taken.push_back(name);
     };
-    struct Reveal { std::string out, index; uint32_t max_length; };
+    struct Reveal { std::string out, index; uint32_t max_length; int reveal; uint32_t salt; };   // salt: index into external_inputs
     std::vector<std::vector<Reveal>> reveals(A.regexes.size());
     for (size_t r = 0; r < A.regexes.size(); ++r) {
         const AppRegex& rx = A.regexes[r];
@@ -943,14 +943,35 @@ Circuit build_email_app(const AppSpec& A, bool materialize_linear) {
         uint32_t q = 0;
         for (size_t i = 0; i < rx.parts.size(); ++i) {
             const AppRegexPart& pt = rx.parts[i];
-            if (!pt.is_public) continue;
-            const std::string pf = field + ".parts[" + std::to_string(i) + "].maxLength";
+            const std::string pfield = field + ".parts[" + std::to_string(i) + "]";
+            if (!pt.is_public) {
+                if (pt.reveal_given) throw std::runtime_error(pfield + ".reveal: only a public part is revealed");
+                if (!pt.salt.empty()) throw std::runtime_error(pfield + ".salt: only a public part with reveal \"commit\" takes a salt");
+                continue;
+            }
+            uint32_t salt = 0;
+            if (pt.reveal == REVEAL_COMMIT) {
+                if (pt.salt.empty()) throw std::runtime_error(pfield + ".salt: reveal \"commit\" needs a salt (a private external input)");
+                bool found = false;
+                for (size_t e = 0; e < A.external_inputs.size() && !found; ++e) {
+                    const AppExternalInput& ei = A.external_inputs[e];
+                    if (ei.name != pt.salt) continue;
+                    found = true;
+                    salt = (uint32_t)e;
+                    if (ei.is_public) throw std::runtime_error(pfield + ".salt: external input '" + pt.salt + "' is public; a salt must be private");
+                    if (ei.max_length) throw std::runtime_error(pfield + ".salt: external input '" + pt.salt + "' is packed; a salt is one field element");
+                }
+                if (!found) throw std::runtime_error(pfield + ".salt: no external input named '" + pt.salt + "'");
+            } else if (!pt.salt.empty()) {
+                throw std::runtime_error(pfield + ".salt: a salt needs reveal \"commit\"");
+            }
+            const std::string pf = pfield + ".maxLength";
             if (pt.max_length == 0) throw std::runtime_error(pf + ": a public part needs maxLength");
             if (pt.max_length > searched)
                 throw std::runtime_error(pf + ": " + std::to_string(pt.max_length) + " is larger than the searched " +
                                          (rx.body ? "body" : "header") + " (" + std::to_string(searched) + " bytes)");
             const std::string base = n_pub == 1 ? rx.name : rx.name + std::to_string(q);
-            reveals[r].push_back(Reveal{base, base + "Index", pt.max_length});
+            reveals[r].push_back(Reveal{base, base + "Index", pt.max_length, pt.reveal, salt});
             ++q;
         }
     }
@@ -975,13 +996,17 @@ Circuit build_email_app(const AppSpec& A, bool materialize_linear) {
     if (!P.ignore_body_hash_check && P.enable_body_masking) masked_body = b.declare_outputs("maskedBody", Bd);
     std::vector<std::vector<std::vector<Var>>> reveal_out(A.regexes.size());
     for (size_t r = 0; r < A.regexes.size(); ++r)
-        for (auto& rv : reveals[r]) reveal_out[r].push_back(b.declare_outputs(rv.out, packed_len(rv.max_length)));
+        for (auto& rv : reveals[r]) reveal_out[r].push_back(b.declare_outputs(rv.out, rv.reveal == REVEAL_BYTES ? packed_len(rv.max_length) : 1));
     Var nullifier = 0;
     if (A.email_nullifier) nullifier = b.declare_outputs("emailNullifier", 1)[0];
 
     auto to_lcs = [](const std::vector<Var>& v) { LCVec o(v.size()); for (size_t i = 0; i < v.size(); ++i) o[i] = LC(v[i]); return o; };
     // public inputs: the app's external inputs, bound to the proof through their public-input rows of the QAP (SURVEY A.7)
-    for (auto& ei : A.external_inputs) b.declare_inputs(ei.name, ei.max_length ? packed_len(ei.max_length) : 1, true);
+    std::vector<Var> external_first(A.external_inputs.size(), 0);
+    for (size_t e = 0; e < A.external_inputs.size(); ++e) {
+        const AppExternalInput& ei = A.external_inputs[e];
+        if (ei.is_public) external_first[e] = b.declare_inputs(ei.name, ei.max_length ? packed_len(ei.max_length) : 1, true)[0];
+    }
     std::vector<Var> pubkey_v;
     if (P.public_pubkey) pubkey_v = b.declare_inputs("pubkey", k, true);
     LCVec email_header = to_lcs(b.declare_inputs("emailHeader", H, false));
@@ -1002,6 +1027,10 @@ Circuit build_email_app(const AppSpec& A, bool materialize_linear) {
     std::vector<std::vector<LC>> reveal_index(A.regexes.size());
     for (size_t r = 0; r < A.regexes.size(); ++r)
         for (auto& rv : reveals[r]) reveal_index[r].push_back(LC(b.declare_inputs(rv.index, 1, false)[0]));
+    for (size_t e = 0; e < A.external_inputs.size(); ++e) {     // private external inputs: after everything else
+        const AppExternalInput& ei = A.external_inputs[e];
+        if (!ei.is_public) external_first[e] = b.declare_inputs(ei.name, ei.max_length ? packed_len(ei.max_length) : 1, false)[0];
+    }
 
     num2bits(b, email_header_length, log2_ceil(H));                      // :58-59
     assert_zero_padding(b, email_header, email_header_length);           // :63
@@ -1068,8 +1097,18 @@ Circuit build_email_app(const AppSpec& A, bool materialize_linear) {
         b.enforce_eq(rx[0], one_lc());                                   // the regex must match
         for (size_t q = 0; q < reveals[r].size(); ++q) {
             LCVec reveal(rx.begin() + 1 + q * msg.size(), rx.begin() + 1 + (q + 1) * msg.size());
-            LCVec packs = pack_regex_reveal(b, reveal, reveal_index[r][q], reveals[r][q].max_length);
-            for (size_t i = 0; i < packs.size(); ++i) b.assign_output(reveal_out[r][q][i], packs[i]);
+            const Reveal& rv = reveals[r][q];
+            LCVec packs = pack_regex_reveal(b, reveal, reveal_index[r][q], rv.max_length);
+            if (rv.reveal == REVEAL_BYTES) {
+                for (size_t i = 0; i < packs.size(); ++i) b.assign_output(reveal_out[r][q][i], packs[i]);
+                continue;
+            }
+            // hash / commit: the packed words stay intermediate signals; the Poseidon instances are recorded for the
+            // engine's native permutation (circuit.hpp: PoseidonBlock)
+            for (LC& p : packs) p = b.signal(p);
+            LC h = poseidon_modular(b, packs, true);
+            if (rv.reveal == REVEAL_COMMIT) h = poseidon(b, {h, LC(external_first[rv.salt])}, true);
+            b.assign_output(reveal_out[r][q][0], h);
         }
     }
     if (A.email_nullifier) b.assign_output(nullifier, email_nullifier(b, n, signature));   // helpers/email-nullifier.circom

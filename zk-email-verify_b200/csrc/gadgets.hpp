@@ -28,7 +28,14 @@ LCVec sha256_compression(Builder& b, const LCVec& hin, const LCVec& inp);   // (
 LCVec sha256_iv_bits();                                                     // H(0..7), LSB-first per word (sha.circom:146-153)
 
 // ---- circomlib poseidon ------------------------------------------------------------------------
-LC poseidon(Builder& b, const LCVec& inputs);                               // Poseidon(n) (utils/hash.circom:38)
+// record: inputs are signals, and the instance gets a PoseidonBlock (circuit.hpp) for native evaluation
+LC poseidon(Builder& b, const LCVec& inputs, bool record = false);          // Poseidon(n) (utils/hash.circom:38)
+struct PoseidonParams {
+    int t, r_f, r_p;
+    std::vector<Fr> rc;                  // (r_f + r_p) * t round constants, round-major
+    std::vector<std::vector<Fr>> mds;    // t x t
+};
+const PoseidonParams& poseidon_params(int t);                               // t = 2..17
 // host-side Poseidon permutation on field elements (used by tests and by the helpers mirror)
 Fr poseidon_hash(const std::vector<Fr>& inputs);
 
@@ -52,7 +59,7 @@ LC clean_email_address(Builder& b, const LCVec& encoded, const LCVec& decoded); 
 LC email_nullifier(Builder& b, uint32_t bits_per_chunk, const LCVec& signature);           // helpers/email-nullifier.circom:14-23
 LCVec select_regex_reveal(Builder& b, const LCVec& in, const LC& start_index, uint32_t max_reveal_len);  // utils/regex.circom:17-52
 LC poseidon_large(Builder& b, uint32_t bits_per_chunk, const LCVec& in);    // utils/hash.circom:15-39
-LC poseidon_modular(Builder& b, const LCVec& in);                           // utils/hash.circom:49-83
+LC poseidon_modular(Builder& b, const LCVec& in, bool record = false);      // utils/hash.circom:49-83
 LC remove_soft_line_breaks(Builder& b, const LCVec& encoded, const LCVec& decoded);   // helpers/remove-soft-line-breaks.circom:14-126 (returns isValid)
 
 // ---- lib/ ------------------------------------------------------------------------------------
@@ -102,14 +109,28 @@ LCVec regex_match_reveals(Builder& b, const std::string& scope, const std::vecto
 // The circuit a zk-email app writes by hand (docs/zk-email-docs/UsageGuide/README.md: write the regex, wrap EmailVerifier,
 // reveal what it matched), built from a description.  TwitterVerifier is the app {body regex twitterUsername, external
 // input address, exposeHeaderHash = false}; EmailVerifier is the app with nothing added.
-struct AppRegexPart { std::string regex; bool is_public = false; uint32_t max_length = 0; };   // max_length: public parts
+// reveal (public parts): the packed bytes as outputs (PackRegexReveal), one output PoseidonModular(packed bytes) (hash), or
+// one output Poseidon(2)([that hash, salt]) with `salt` a private one-element external input (commit)
+enum AppReveal { REVEAL_BYTES = 0, REVEAL_HASH = 1, REVEAL_COMMIT = 2 };
+struct AppRegexPart {
+    std::string regex;
+    bool is_public = false;
+    uint32_t max_length = 0;           // public parts
+    int reveal = REVEAL_BYTES;
+    bool reveal_given = false;         // the spec named a reveal (refused on a part that is not public)
+    std::string salt;                  // REVEAL_COMMIT: the external input holding the salt
+};
 struct AppRegex {
     std::string name;
     bool body = false;                 // search emailBody (decodedEmailBodyIn with removeSoftLineBreaks), else emailHeader
     std::vector<AppRegexPart> parts;
     std::string scope;                 // scope of its constraints (default: name)
 };
-struct AppExternalInput { std::string name; uint32_t max_length = 0; };   // 0: one field element, else PackBytes layout
+struct AppExternalInput {
+    std::string name;
+    uint32_t max_length = 0;           // 0: one field element, else PackBytes layout
+    bool is_public = true;             // private inputs follow the start indices of the public parts
+};
 struct AppSpec {
     EmailVerifierParams ev;            // ev.twitter is ignored
     bool expose_header_hash = true;

@@ -108,12 +108,43 @@ Fr poseidon_hash(const std::vector<Fr>& inputs) {
     return st[0];
 }
 
-LC poseidon(Builder& b, const LCVec& inputs) {
+const PoseidonParams& poseidon_params(int t) {
+    static std::map<int, PoseidonParams> cache;
+    auto it = cache.find(t);
+    if (it != cache.end()) return it->second;
+    const Params& P = params_for(t);
+    PoseidonParams q;
+    q.t = t;
+    q.r_f = R_F;
+    q.r_p = P.r_p;
+    q.rc = P.rc;
+    q.mds = P.mds;
+    return cache.emplace(t, std::move(q)).first->second;
+}
+
+LC poseidon(Builder& b, const LCVec& inputs, bool record) {
     ScopeGuard g(b, "Poseidon");
     const int t = (int)inputs.size() + 1;
     const Params& P = params_for(t);
+    PoseidonBlock blk;
+    if (record) {
+        blk.t = (uint32_t)t;
+        for (const LC& in : inputs) {
+            Var v;
+            if (!in.is_single_var(&v)) throw std::runtime_error("Poseidon record: every input must be a signal");
+            blk.inputs.push_back(v);
+        }
+        blk.var_begin = b.num_vars();
+        blk.temp_begin = b.num_temps();
+    }
+    // a signal the gadget created for (round, lane, kind) gets its descriptor (constants and aliases create none)
+    auto note = [&](const LC& e, int rnd, int lane, uint32_t kind) {
+        Var v;
+        if (record && e.is_single_var(&v) && v >= blk.var_begin)
+            blk.desc.insert(blk.desc.end(), {v, (uint32_t)rnd << 16 | (uint32_t)lane << 8 | kind});
+    };
     LCVec st(t);
-    for (int i = 1; i < t; ++i) st[i] = b.signal(inputs[i - 1]);
+    for (int i = 1; i < t; ++i) { st[i] = b.signal(inputs[i - 1]); note(st[i], 0, i, POS_K_INPUT); }
     int k = 0;
     const int rounds = R_F + P.r_p;
     for (int rnd = 0; rnd < rounds; ++rnd) {
@@ -125,6 +156,7 @@ LC poseidon(Builder& b, const LCVec& inputs) {
             LC x2 = b.mul(x, x);
             LC x4 = b.mul(x2, x2);
             st[i] = b.mul(x4, x);
+            note(x2, rnd, i, POS_K_X2); note(x4, rnd, i, POS_K_X4); note(st[i], rnd, i, POS_K_X5);
         }
         LCVec nx(t);                                                          // Mix
         for (int i = 0; i < t; ++i) {
@@ -132,8 +164,15 @@ LC poseidon(Builder& b, const LCVec& inputs) {
             for (int j = 0; j < t; ++j) e += st[j] * P.mds[i][j];
             // only state[0] is the hash output; it is enough to materialise what later rounds consume
             nx[i] = (rnd == rounds - 1 && i != 0) ? LC() : b.signal(e);
+            if (!(rnd == rounds - 1 && i != 0)) note(nx[i], rnd, i, POS_K_MIX);
         }
         st.swap(nx);
+    }
+    if (record) {
+        blk.var_end = b.num_vars();
+        blk.temp_end = b.num_temps();
+        if (blk.desc.size() / 2 != blk.var_end - blk.var_begin) throw std::runtime_error("Poseidon record: a created signal has no descriptor");
+        b.add_poseidon_block(std::move(blk));
     }
     return st[0];
 }

@@ -411,6 +411,52 @@ __device__ void fpmul_coop(const DevProgram& P, uint8_t* w, uint32_t aux_off, ui
     __syncthreads();
 }
 
+// ---- native Poseidon (circuit.hpp: PoseidonBlock) ---------------------------------------------------------------------
+// The gadget's signals are the lanes of one permutation's state round by round; walked as ops they are ~4 dependency
+// levels per round (x^2, x^4, x^5, mix), each holding a handful of ops.  Here ONE WARP runs the whole permutation: lane i
+// holds state element i (t <= 17) in standard form, full rounds run the S-box on every lane and partial rounds on lane 0,
+// the mix gathers the state with shuffles, and every lane writes the signals the gadget created for it (the slot table of
+// witness_program.hpp: POSEIDON_AUX; slot 0 = no signal).  The CPU oracle walks the gadget's own ops, so "GPU witness ==
+// oracle witness" checks this path; tests/test_app_commit.py checks the record on the CPU.
+__device__ __forceinline__ void put_signal(uint8_t* w, uint32_t var, const Fr& x) { if (var) x.store(w + 32ull * var); }
+
+__device__ void poseidon_coop(const DevProgram& P, uint8_t* w, uint32_t aux_off) {
+    const uint32_t lane = threadIdx.x & 31u;
+    const uint32_t* ax = P.aux + aux_off;
+    const uint32_t t = ax[0], r_p = ax[1], rounds = 8 + r_p;
+    const uint32_t* rc = P.aux + ax[2];              // [rounds][t] standard form, 8 words each
+    const uint32_t* mds = rc + 8 * rounds * t;       // [t][t] times R
+    const uint32_t* in = ax + 3;
+    const uint32_t* slot = in + (t - 1);
+    const bool on = lane < t;
+    Fr st = Fr::zero();
+    if (on && lane > 0) { st = Fr::load(w + 32ull * in[lane - 1]); put_signal(w, slot[lane], st); }
+#pragma unroll 1
+    for (uint32_t r = 0; r < rounds; ++r) {
+        const uint32_t* sl = slot + t + 4 * (r * t + lane);
+        if (on) {
+            st = st + Fr::load(rc + 8 * (r * t + lane));
+            if (lane == 0 || r < 4 || r >= 4 + r_p) {   // S-box: x^5 from xR = x (x) R^2 as x^2 = xR (x) x, x^4 = x^2 R (x) x^2
+                const Fr xr = st * Fr::r2();
+                const Fr x2 = xr * st, x2r = xr * xr;
+                const Fr x4 = x2r * x2;
+                st = x4 * xr;
+                put_signal(w, sl[0], x2); put_signal(w, sl[1], x4); put_signal(w, sl[2], st);
+            }
+        }
+        Fr acc = Fr::zero();
+#pragma unroll 1
+        for (uint32_t j = 0; j < t; ++j) {
+            Fr sj;
+#pragma unroll
+            for (int q = 0; q < 8; ++q) sj.v[q] = __shfl_sync(0xffffffffu, st.v[q], (int)j);
+            if (on) acc = acc + Fr::load(mds + 8 * (lane * t + j)) * sj;
+        }
+        st = acc;
+        if (on) put_signal(w, sl[3], st);
+    }
+}
+
 __device__ __forceinline__ void cp_async16(void* smem_dst, const void* gmem_src) {
     const uint32_t d = (uint32_t)__cvta_generic_to_shared(smem_dst);
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d), "l"(gmem_src) : "memory");
@@ -505,11 +551,20 @@ witness_kernel(DevProgram P, uint8_t* __restrict__ w_all, size_t stride_elems, c
         } else if (code == 4) {   // OP_FPMUL
             fpmul_hint_dev(P, w, op.z, op.x);
         }
-        // cooperative ops of this iteration (native Sha256compression): the whole CTA works on each in turn; they only
+        // cooperative ops of this iteration (native Sha256compression, regex seeds, FpMul hints): the whole CTA works on each in
+        // turn, native Poseidon instances on a warp each; they only
         // read signals of earlier levels and define signals nothing else in this iteration touches
-        for (uint32_t q = 0; q < (hdr.w & 0xffffu); ++q) {
+        const uint32_t n_coop = hdr.w & 0xffffu;
+        for (uint32_t q = 0; q < n_coop; ++q) {
             const uint32_t c0 = P.coop[2 * (hdr.z + q)], c1 = P.coop[2 * (hdr.z + q) + 1];
-            if (c0 >> 31) fpmul_coop(P, w, c0 & 0x7fffffffu, c1, fpmul_s);
+            if ((c0 >> 30) == 3u) {          // a run of native Poseidon instances (the level's last coop ops): one warp each
+                uint32_t e = q + 1;
+                while (e < n_coop && (P.coop[2 * (hdr.z + e)] >> 30) == 3u) ++e;
+                for (uint32_t p = q + tid / 32u; p < e; p += WITNESS_THREADS / 32) poseidon_coop(P, w, P.coop[2 * (hdr.z + p)] & 0x3fffffffu);
+                __syncthreads();
+                q = e - 1;
+            }
+            else if (c0 >> 31) fpmul_coop(P, w, c0 & 0x7fffffffu, c1, fpmul_s);
             else if (c0 & 0x40000000u) regex_coop(P, w, c0 & 0x3fffffffu, sha_q);
             else sha_coop(P, w, c0, sha_q, sha_in);
         }

@@ -1,6 +1,8 @@
 // Lowering of the levelised witness program into the witness kernel's stream (witness_program.hpp).
 #include "witness_program.hpp"
+#include "gadgets.hpp"
 #include <algorithm>
+#include <map>
 #include <stdexcept>
 
 namespace zke {
@@ -29,13 +31,15 @@ std::vector<uint32_t> coef_words(const std::vector<U256>& coefs) {
 
 namespace {
 
-const uint32_t XOP_SHA = 6, XOP_RX = 7;
+const uint32_t XOP_SHA = 6, XOP_RX = 7, XOP_POS = 8;
 
 struct Levelised {
-    std::vector<WOp> xops;                         // code XOP_SHA: a = index of the block; XOP_RX: a = index of the seed
+    std::vector<WOp> xops;                         // code XOP_SHA: a = index of the block; XOP_RX: a = index of the seed;
+                                                   // XOP_POS: a = index of the Poseidon block
     std::vector<uint32_t> xlevel_ptr;              // ops of level l: [xlevel_ptr[l], xlevel_ptr[l + 1])
-    std::vector<uint32_t> aux;                     // the circuit's aux table, then the regex seed images and the SHA tables
-    std::vector<uint32_t> sha_aux_off, rx_aux_off; // per block / seed: offset of its table in aux
+    std::vector<uint32_t> aux;                     // the circuit's aux table, then the regex seed images, the SHA tables and
+                                                   // the Poseidon tables and constants
+    std::vector<uint32_t> sha_aux_off, rx_aux_off, pos_aux_off; // per block / seed: offset of its table in aux
 };
 
 // ---- native Sha256compression (circuit.hpp: ShaBlock): the ops that define the signals / scratch slots of a recorded
@@ -45,16 +49,19 @@ struct Levelised {
 // message and writes every state signal; the instance's own ops stay (they write the same values again) but now depend on
 // seeded signals instead of on the previous position's gadgets, so the ~4 levels per message byte collapse into a handful
 // for the whole message.
-Levelised substitute_and_levelise(const Circuit& c, bool native_sha, bool native_rx) {
+// ---- native Poseidon (circuit.hpp: PoseidonBlock): as for SHA, the gadget's ops are replaced by one cooperative op per
+// instance - a Poseidon(t - 1) costs one level instead of ~4 per round (~260 for the widths of a PoseidonModular).
+Levelised substitute_and_levelise(const Circuit& c, bool native_sha, bool native_rx, bool native_pos) {
     Levelised L;
     std::vector<WOp>& xops = L.xops;
     std::vector<uint32_t>& xlevel_ptr = L.xlevel_ptr;
     std::vector<uint32_t>& aux = L.aux;
-    std::vector<uint32_t>& sha_aux_off = L.sha_aux_off, &rx_aux_off = L.rx_aux_off;
+    std::vector<uint32_t>& sha_aux_off = L.sha_aux_off, &rx_aux_off = L.rx_aux_off, &pos_aux_off = L.pos_aux_off;
     aux = c.aux;
     sha_aux_off.assign(c.sha_blocks.size(), 0);
     rx_aux_off.assign(c.regex_seeds.size(), 0);
-    if (!native_sha && !native_rx) {
+    pos_aux_off.assign(c.poseidon_blocks.size(), 0);
+    if (!native_sha && !native_rx && !native_pos) {
         xops = c.ops;
         xlevel_ptr = c.level_ptr;
         return L;
@@ -79,6 +86,35 @@ Levelised substitute_and_levelise(const Circuit& c, bool native_sha, bool native
         aux.insert(aux.end(), B.inputs.begin(), B.inputs.end());
         aux.insert(aux.end(), B.desc.begin(), B.desc.end());
     }
+    if (native_pos) {
+        std::map<uint32_t, uint32_t> consts_off;       // width -> offset of its constants
+        for (const PoseidonBlock& B : c.poseidon_blocks) {
+            if (consts_off.count(B.t)) continue;
+            const gadgets::PoseidonParams& Pp = gadgets::poseidon_params((int)B.t);
+            while (aux.size() % 8) aux.push_back(0);   // 32-byte rows: the device loads them as two 16-byte words
+            consts_off[B.t] = (uint32_t)aux.size();
+            for (const Fr& x : Pp.rc) { const U256 u = x.to_u256(); for (int q = 0; q < 4; ++q) aux.insert(aux.end(), {(uint32_t)u.v[q], (uint32_t)(u.v[q] >> 32)}); }
+            for (auto& row : Pp.mds) for (const Fr& x : row) for (int q = 0; q < 4; ++q) aux.insert(aux.end(), {(uint32_t)x.m.v[q], (uint32_t)(x.m.v[q] >> 32)});
+        }
+        for (size_t bi = 0; bi < c.poseidon_blocks.size(); ++bi) {
+            const PoseidonBlock& B = c.poseidon_blocks[bi];
+            const gadgets::PoseidonParams& Pp = gadgets::poseidon_params((int)B.t);
+            if (B.inputs.size() + 1 != B.t) throw std::runtime_error("native Poseidon: a record's inputs do not match its width");
+            for (uint32_t v = B.var_begin; v < B.var_end; ++v) owner[v] = (int32_t)bi;
+            for (uint32_t v = B.temp_begin; v < B.temp_end; ++v) owner[v] = (int32_t)bi;
+            pos_aux_off[bi] = (uint32_t)aux.size();
+            aux.insert(aux.end(), {B.t, (uint32_t)Pp.r_p, consts_off[B.t]});
+            aux.insert(aux.end(), B.inputs.begin(), B.inputs.end());
+            const size_t slots = aux.size(), rounds = (size_t)(Pp.r_f + Pp.r_p);
+            aux.resize(slots + B.t + rounds * B.t * 4, 0);
+            for (size_t d = 0; d < B.desc.size(); d += 2) {
+                const uint32_t rnd = B.desc[d + 1] >> 16, lane = (B.desc[d + 1] >> 8) & 0xff, kind = B.desc[d + 1] & 0xff;
+                if (rnd >= rounds || lane >= B.t || kind > POS_K_MIX || (kind == POS_K_INPUT && rnd != 0)) throw std::runtime_error("native Poseidon: bad descriptor");
+                aux[slots + (kind == POS_K_INPUT ? lane : B.t + ((size_t)rnd * B.t + lane) * 4 + kind - 1)] = B.desc[d];
+            }
+        }
+        if (aux.size() >= (1u << 30)) throw std::runtime_error("witness program: auxiliary table too large");
+    }
     // Order: c.ops is in level order (producers before consumers).  A block's op is inserted right after the
     // producer of its LAST-defined input: everything it reads precedes it, and everything that reads its outputs
     // (the final-sum bits, originally defined after all of the block's inputs) follows it.
@@ -88,7 +124,12 @@ Levelised substitute_and_levelise(const Circuit& c, bool native_sha, bool native
         const uint32_t nd = o.code == OP_FPMUL ? 2 * c.aux[o.a + 1] : 1;
         for (uint32_t j = 0; j < nd; ++j) def_pos[o.dst + j] = (int64_t)i;
     }
-    std::vector<std::vector<uint32_t>> blocks_at(c.ops.size() + 1), seeds_at(c.ops.size() + 1);
+    std::vector<std::vector<uint32_t>> blocks_at(c.ops.size() + 1), seeds_at(c.ops.size() + 1), pos_at(c.ops.size() + 1);
+    for (size_t bi = 0; native_pos && bi < c.poseidon_blocks.size(); ++bi) {
+        int64_t pos = 0;
+        for (uint32_t v : c.poseidon_blocks[bi].inputs) pos = std::max(pos, def_pos[v] + 1);
+        pos_at[(size_t)pos].push_back((uint32_t)bi);
+    }
     for (size_t bi = 0; native_sha && bi < c.sha_blocks.size(); ++bi) {
         int64_t pos = 0;
         for (uint32_t v : c.sha_blocks[bi].inputs) if (v < SHA_CONST0) pos = std::max(pos, def_pos[v] + 1);
@@ -104,6 +145,7 @@ Levelised substitute_and_levelise(const Circuit& c, bool native_sha, bool native
     for (size_t i = 0; i <= c.ops.size(); ++i) {
         for (uint32_t bi : blocks_at[i]) kept.push_back(WOp{XOP_SHA, c.sha_blocks[bi].var_begin, bi, 0, 0});
         for (uint32_t ri : seeds_at[i]) kept.push_back(WOp{XOP_RX, 0, ri, 0, 0});
+        for (uint32_t pi : pos_at[i]) kept.push_back(WOp{XOP_POS, 0, pi, 0, 0});
         if (i < c.ops.size() && owner[c.ops[i].dst] < 0) kept.push_back(c.ops[i]);
     }
     // levelise (the same rules as Builder::finalize, plus the multi-output block op)
@@ -112,7 +154,7 @@ Levelised substitute_and_levelise(const Circuit& c, bool native_sha, bool native
     defined[0] = 1;
     for (auto& g : c.groups) if (g.kind != 0) for (uint32_t i = 0; i < g.count; ++i) defined[g.first + i] = 1;
     auto need = [&](uint32_t v) -> uint32_t {
-        if (!defined[v]) throw std::runtime_error("native SHA substitution: an op reads an unassigned signal");
+        if (!defined[v]) throw std::runtime_error("native op substitution: an op reads an unassigned signal");
         return level[v];
     };
     auto lc_level = [&](uint32_t id) { uint32_t l = 0; for (uint32_t k = c.lc_ptr[id]; k < c.lc_ptr[id + 1]; ++k) l = std::max(l, need(c.lc_var[k])); return l; };
@@ -127,6 +169,7 @@ Levelised substitute_and_levelise(const Circuit& c, bool native_sha, bool native
             case OP_FPMUL: { const uint32_t kk = c.aux[o.a + 1]; for (uint32_t j = 0; j < 3 * kk; ++j) l = std::max(l, need(c.aux[o.a + 2 + j])); break; }
             case XOP_SHA: for (uint32_t v : c.sha_blocks[o.a].inputs) if (v < SHA_CONST0) l = std::max(l, need(v)); break;
             case XOP_RX: for (uint32_t v : c.regex_seeds[o.a].bytes) l = std::max(l, need(v)); break;
+            case XOP_POS: for (uint32_t v : c.poseidon_blocks[o.a].inputs) l = std::max(l, need(v)); break;
             default: throw std::runtime_error("bad opcode");
         }
         l += 1;
@@ -136,6 +179,9 @@ Levelised substitute_and_levelise(const Circuit& c, bool native_sha, bool native
         } else if (o.code == XOP_RX) {
             const RegexSeed& R = c.regex_seeds[o.a];
             for (size_t d = 0; d < R.desc.size(); d += 2) { defined[R.desc[d]] = 1; level[R.desc[d]] = l; }
+        } else if (o.code == XOP_POS) {
+            const PoseidonBlock& B = c.poseidon_blocks[o.a];
+            for (size_t d = 0; d < B.desc.size(); d += 2) { defined[B.desc[d]] = 1; level[B.desc[d]] = l; }
         } else if (o.code == OP_FPMUL) {
             const uint32_t kk = c.aux[o.a + 1];
             for (uint32_t j = 0; j < 2 * kk; ++j) { defined[o.dst + j] = 1; level[o.dst + j] = l; }
@@ -184,12 +230,15 @@ std::vector<std::pair<size_t, size_t>> stream_levels(const Circuit& c, const std
         const size_t level_first_iter = hdr.size() / 4;
         order.clear();
         const uint32_t coop_first = (uint32_t)(coop.size() / 2);
+        std::vector<uint32_t> pos_coop;                // after the level's other cooperative ops: adjacent, one warp each
         for (uint32_t i = beg; i < end; ++i) {
-            if (xops[i].code == XOP_SHA) { coop.push_back(L.sha_aux_off[xops[i].a]); coop.push_back(0); }
+            if (xops[i].code == XOP_POS) { pos_coop.push_back(0xc0000000u | L.pos_aux_off[xops[i].a]); pos_coop.push_back(0); }
+            else if (xops[i].code == XOP_SHA) { coop.push_back(L.sha_aux_off[xops[i].a]); coop.push_back(0); }
             else if (xops[i].code == XOP_RX) { coop.push_back(0x40000000u | L.rx_aux_off[xops[i].a]); coop.push_back(0); }
             else if (xops[i].code == OP_FPMUL && coop_fpmul) { coop.push_back(0x80000000u | xops[i].a); coop.push_back(xops[i].dst); }
             else order.push_back(i);
         }
+        coop.insert(coop.end(), pos_coop.begin(), pos_coop.end());
         uint32_t coop_left = (uint32_t)(coop.size() / 2) - coop_first;   // attached to the level's first iteration
         // Sort key: kind, then the positions of the terms that need a product (coefficient other than +-1) in the
         // flattened [A | B | C] term list, then the term count.  Within an LC the product terms are emitted first
@@ -301,7 +350,8 @@ WitnessStream lower_witness_program(const Circuit& c, const std::vector<uint32_t
     // instances here instead of producing a witness that fails its constraints later
     for (const WOp& o : c.ops)
         if (o.code == OP_FPMUL && c.aux[o.a + 1] > 20) throw std::runtime_error("FpMul with k = " + std::to_string(c.aux[o.a + 1]) + " limbs exceeds the device hint's limit of 20");
-    Levelised L = substitute_and_levelise(c, opt.native_sha && !c.sha_blocks.empty(), opt.native_regex && !c.regex_seeds.empty());
+    Levelised L = substitute_and_levelise(c, opt.native_sha && !c.sha_blocks.empty(), opt.native_regex && !c.regex_seeds.empty(),
+                                          opt.native_poseidon && !c.poseidon_blocks.empty());
     WitnessStream S;
     const std::vector<std::pair<size_t, size_t>> level_iters = stream_levels(c, coef_word, L, opt.coop_fpmul, opt.cluster, S);
     S.aux = std::move(L.aux);

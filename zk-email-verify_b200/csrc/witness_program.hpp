@@ -28,6 +28,7 @@ std::vector<uint32_t> coef_words(const std::vector<U256>& coefs);
 struct LowerOptions {
     bool native_sha = true;      // one cooperative op per recorded Sha256compression instead of the gadget's own ops
     bool native_regex = true;    // one cooperative op per zk-regex instance seeds its state signals
+    bool native_poseidon = true; // one cooperative op per recorded Poseidon instance instead of the gadget's own ops
     bool coop_fpmul = true;      // FpMul hints as cooperative ops (false: the sequential single-thread hint, a regular record)
     uint32_t cluster = 1;        // CTAs per email (1, 2, 4, 8): every level is padded to whole rounds of `cluster` iterations
 };
@@ -42,7 +43,13 @@ struct WitnessStream {
     std::vector<uint32_t> coop;        // cooperative ops of the iterations (executed by the whole CTA), two words each:
                                        // {offset into `aux`, 0}: native Sha256compression table ({n_desc, inputs[768],
                                        // desc[n_desc][2]}, circuit.hpp: ShaBlock); {1 << 30 | offset into `aux`, 0}: regex seed
-                                       // (circuit.hpp: regex_flat image of one seed); {1 << 31 | offset into `aux`, dst}: FpMul hint
+                                       // (circuit.hpp: regex_flat image of one seed); {1 << 31 | offset into `aux`, dst}: FpMul hint;
+                                       // {3 << 30 | offset into `aux`, 0}: native Poseidon (POSEIDON_AUX below) - the Poseidon ops of
+                                       // an iteration are adjacent and run side by side, one warp each
+    // native Poseidon in `aux`: per instance {t, r_p, offset of the width's constants, inputs[t - 1], slots[t + (8 + r_p) t 4]}
+    // (slots: the signal of each lane's input copy, then per round and lane the signals of x^2, x^4, x^5 and the mix output;
+    // 0 = the gadget created none), per width once, 8-word aligned: round constants [(8 + r_p) t] in standard form, then the
+    // MDS matrix [t][t] times R (the coefficient form of lc_term.cuh: a Montgomery product with it gives the plain product)
     std::vector<uint32_t> iter_info;   // per iteration {first op's record word 1, live ops, terms} (diagnostics: ZKE_WITNESS_TRACE)
     std::vector<uint32_t> level_ops;   // per level: records that are not cooperative ops
     uint32_t n_iters = 0, n_levels = 0, cluster = 1;

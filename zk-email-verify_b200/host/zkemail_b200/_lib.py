@@ -54,6 +54,10 @@ zke_circuit_array = _sig("zke_circuit_array", c_void_p, [c_void_p, c_int, ctypes
 zke_circuit_scope_name = _sig("zke_circuit_scope_name", c_char_p, [c_void_p, c_u32])
 zke_circuit_program_stats = _sig("zke_circuit_program_stats", c_int, [c_void_p, c_int, c_int, c_int, c_u32, ctypes.POINTER(ProgramStats),
                                                                       ctypes.POINTER(c_u32), c_size_t, c_char_p, c_size_t])
+zke_circuit_program_stats_ex = _sig("zke_circuit_program_stats_ex", c_int, [c_void_p, c_u32, c_u32, ctypes.POINTER(ProgramStats),
+                                                                            ctypes.POINTER(c_u32), c_size_t, c_char_p, c_size_t])
+LOWER_NATIVE_SHA, LOWER_NATIVE_REGEX, LOWER_COOP_FPMUL, LOWER_NATIVE_POSEIDON = 1, 2, 4, 8
+zke_poseidon_hash = _sig("zke_poseidon_hash", c_int, [c_char_p, c_size_t, c_char_p])
 zke_device_count = _sig("zke_device_count", c_int, [])
 zke_version = _sig("zke_version", c_char_p, [])
 
@@ -62,6 +66,7 @@ zke_version = _sig("zke_version", c_char_p, [])
  ARR_OPS, ARR_LEVEL_PTR, ARR_LC_PTR, ARR_LC_VAR, ARR_LC_COEF, ARR_AUX, ARR_SCOPE_OF_CONSTRAINT) = range(17)
 ARR_SHA_BLOCKS = 17
 ARR_REGEX_SEEDS = 18
+ARR_POSEIDON_BLOCKS = 19
 
 
 class ZkeError(RuntimeError):

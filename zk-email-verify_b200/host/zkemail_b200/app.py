@@ -16,7 +16,17 @@ the regex, wrap EmailVerifier, reveal what it matched as public outputs):
 
 Every public part of a regex becomes a PackRegexReveal output of ceil(maxLength / 31) field elements, named after the
 regex (`name`, or `name0`, `name1`, ... when the regex has several public parts), with a private start-index input
-(`nameIndex` / `name0Index`, ...)."""
+(`nameIndex` / `name0Index`, ...).
+
+A public part may instead publish a hash of what it matched, with `"reveal"`:
+
+    {"regexDef": "[a-z0-9.]+@[a-z0-9.]+", "isPublic": true, "maxLength": 64, "reveal": "hash"}
+        one output: PoseidonModular(PackBytes(part, maxLength)) - poseidon_modular(pack_bytes(part, maxLength))
+    {"regexDef": "...", "isPublic": true, "maxLength": 64, "reveal": "commit", "salt": "senderSalt"}
+        one output: Poseidon(2)([that hash, salt]), the salt a private external input {"name": "senderSalt", "isPublic": false}
+
+`"reveal": "bytes"` is the default.  External inputs are public unless `"isPublic": false`; private ones come after the
+start indices in the witness.  expected_app_output gives the value a verifier compares an output with."""
 from __future__ import annotations
 import re
 
@@ -37,6 +47,32 @@ def public_parts(regex: dict) -> list[tuple[int, str, int]]:
     pub = [(i, p) for i, p in enumerate(regex["parts"]) if p.get("isPublic")]
     name = regex["name"]
     return [(i, name if len(pub) == 1 else f"{name}{q}", int(p["maxLength"])) for q, (i, p) in enumerate(pub)]
+
+
+def _reveal(regex: dict, index: int) -> str:
+    return regex["parts"][index].get("reveal", "bytes")
+
+
+def expected_app_output(spec: dict, name: str, value_bytes, salt=None) -> int | str:
+    """The value the app output `name` holds when its part matched `value_bytes`: the string itself for a plain reveal,
+    poseidon_modular(pack_bytes(value, maxLength)) for `"reveal": "hash"`, and Poseidon(2)([that hash, salt]) for
+    `"reveal": "commit"` - what a verifier who knows the value (and the salt) compares the public signal with."""
+    from .hash import poseidon, poseidon_modular
+    data = value_bytes.encode("utf-8") if isinstance(value_bytes, str) else bytes(value_bytes)
+    for rx in spec.get("regexes", []):
+        for i, out, max_length in public_parts(rx):
+            if out != name:
+                continue
+            mode = _reveal(rx, i)
+            if mode == "bytes":
+                return data.decode("utf-8", errors="replace")
+            h = poseidon_modular(int(x) for x in pack_bytes(data, max_length))
+            if mode == "hash":
+                return h
+            if salt is None:
+                raise ValueError(f'output "{name}" is a commitment: the salt is needed')
+            return poseidon([h, int(salt, 0) if isinstance(salt, str) else int(salt)])
+    raise ValueError(f'the spec has no revealed part named "{name}"')
 
 
 def pack_bytes(data: bytes, max_length: int) -> list[str]:
@@ -63,8 +99,8 @@ def generate_app_inputs(raw_email_or_dkim_result, spec: dict, external_inputs: d
                         params: dict | None = None) -> dict:
     """Circuit inputs of an app circuit: the EmailVerifier inputs (with the spec's flags and shaPrecomputeSelector), the
     start index of every public part - found by running the same decomposed regex through Python `re` on the array the
-    circuit searches (emailHeader, emailBody or decodedEmailBodyIn) - and the external inputs (strings with a maxLength
-    are packed, everything else is one field element).  `params` may add headerMask / bodyMask and, for a raw email, a
+    circuit searches (emailHeader, emailBody or decodedEmailBodyIn) - and the external inputs, private ones (salts)
+    included (strings with a maxLength are packed, everything else is one field element).  `params` may add headerMask / bodyMask and, for a raw email, a
     DKIM key `resolver`.  Raises ValueError naming the regex that does not match."""
     params = dict(params or {})
     resolver = params.pop("resolver", None)
@@ -104,7 +140,8 @@ def generate_app_inputs(raw_email_or_dkim_result, spec: dict, external_inputs: d
 
 def decode_app_outputs(spec: dict, public_signals) -> dict:
     """Public signals of an app proof (snarkjs public.json order) -> {name: value}: revealed substrings and packed
-    external inputs as strings, every other signal as an int (the masks as lists of byte values)."""
+    external inputs as strings, every other signal as an int (hashed and committed parts included; the masks as lists of
+    byte values).  Private external inputs are not public signals."""
     sig = [int(x) for x in public_signals]
     pos = 0
 
@@ -125,11 +162,16 @@ def decode_app_outputs(spec: dict, public_signals) -> dict:
     if not spec.get("ignoreBodyHashCheck") and spec.get("enableBodyMasking"):
         out["maskedBody"] = take(Bd)
     for rx in spec.get("regexes", []):
-        for _, name, max_length in public_parts(rx):
-            out[name] = unpack_bytes(take(_chunks(max_length))).decode("utf-8", errors="replace")
+        for i, name, max_length in public_parts(rx):
+            if _reveal(rx, i) == "bytes":
+                out[name] = unpack_bytes(take(_chunks(max_length))).decode("utf-8", errors="replace")
+            else:
+                out[name] = take(1)[0]
     if spec.get("emailNullifier"):
         out["emailNullifier"] = take(1)[0]
     for ei in spec.get("externalInputs", []):
+        if not ei.get("isPublic", True):
+            continue
         if "maxLength" in ei:
             out[ei["name"]] = unpack_bytes(take(_chunks(int(ei["maxLength"])))).decode("utf-8", errors="replace")
         else:
@@ -141,4 +183,4 @@ def decode_app_outputs(spec: dict, public_signals) -> dict:
     return out
 
 
-__all__ = ["generate_app_inputs", "decode_app_outputs", "pack_bytes", "unpack_bytes", "public_parts"]
+__all__ = ["generate_app_inputs", "decode_app_outputs", "expected_app_output", "pack_bytes", "unpack_bytes", "public_parts"]

@@ -124,15 +124,16 @@ class Circuit:
         p = L.zke_circuit_array(self._h, which, ctypes.byref(n))
         return p, n.value
 
-    def program_stats(self, native_sha=True, native_regex=True, coop_fpmul=True, cluster=1) -> dict:
+    def program_stats(self, native_sha=True, native_regex=True, coop_fpmul=True, cluster=1, native_poseidon=True) -> dict:
         """What the engine's lowering of the witness program (csrc/witness_program.cpp) builds for these options, computed
         on the host: the fields of zke_program_stats plus `level_ops`, the records per level that are not cooperative ops."""
         st, err = L.ProgramStats(), ctypes.create_string_buffer(L.ERRCAP)
+        flags = ((L.LOWER_NATIVE_SHA if native_sha else 0) | (L.LOWER_NATIVE_REGEX if native_regex else 0) |
+                 (L.LOWER_COOP_FPMUL if coop_fpmul else 0) | (L.LOWER_NATIVE_POSEIDON if native_poseidon else 0))
         cap = max(1, self.info.n_levels)
         while True:                # the first min(n_levels, cap) levels are written: once more if the program got deeper
             level_ops = (L.c_u32 * cap)()
-            if L.zke_circuit_program_stats(self._h, int(native_sha), int(native_regex), int(coop_fpmul), cluster, ctypes.byref(st),
-                                           level_ops, cap, err, L.ERRCAP) != 0:
+            if L.zke_circuit_program_stats_ex(self._h, flags, cluster, ctypes.byref(st), level_ops, cap, err, L.ERRCAP) != 0:
                 raise L.ZkeError(err.value.decode())
             if st.n_levels <= cap:
                 break

@@ -1,0 +1,48 @@
+"""Poseidon hashes of the helpers package (packages/helpers/src/hash.ts), on the library's host permutation
+(zke_poseidon_hash: circomlib's parameters, the permutation the circuits constrain).
+
+    poseidon(inputs)                                  Poseidon(n) of 1..16 field elements
+    poseidon_large(value, num_chunks, bits_per_chunk) poseidonLarge: the little-endian chunks of value, hashed once
+    poseidon_modular(inputs)                          poseidonModular: chunks of 16 hashed, the chunk hashes folded left
+                                                      to right with Poseidon(2) - the PoseidonModular template
+
+Inputs are reduced modulo r as circomlibjs does; outputs are ints below r."""
+from __future__ import annotations
+import ctypes
+
+from . import _lib as L
+from .binary_format import bigint_to_chunked_bytes
+from .circuit import FR_MODULUS
+
+CHUNK_SIZE = 16
+
+
+def poseidon(inputs) -> int:
+    """circomlib Poseidon(len(inputs)): state [0, inputs...], output state[0] after the permutation."""
+    vals = [int(x) % FR_MODULUS for x in inputs]
+    if not 1 <= len(vals) <= CHUNK_SIZE:
+        raise ValueError(f"Poseidon takes 1 to {CHUNK_SIZE} inputs, not {len(vals)}")
+    out = ctypes.create_string_buffer(32)
+    if L.zke_poseidon_hash(b"".join(v.to_bytes(32, "little") for v in vals), len(vals), out) != 0:
+        raise L.ZkeError("zke_poseidon_hash failed")
+    return int.from_bytes(out.raw, "little")
+
+
+def poseidon_large(value: int, num_chunks: int, bits_per_chunk: int) -> int:
+    """poseidonLarge(input, numChunks, bitsPerChunk): Poseidon of the num_chunks little-endian bits_per_chunk-bit chunks."""
+    return poseidon([int(x) for x in bigint_to_chunked_bytes(int(value), bits_per_chunk, num_chunks)])
+
+
+def poseidon_modular(inputs) -> int:
+    """poseidonModular(inputs): what an app circuit's `"reveal": "hash"` output holds for the packed bytes of the part."""
+    vals = [int(x) for x in inputs]
+    out = None
+    for start in range(0, len(vals), CHUNK_SIZE):
+        h = poseidon(vals[start:start + CHUNK_SIZE])
+        out = h if out is None else poseidon([out, h])
+    if out is None:
+        raise ValueError("No inputs provided")
+    return out
+
+
+__all__ = ["poseidon", "poseidon_large", "poseidon_modular"]

@@ -22,6 +22,8 @@ const zke_agg_bytes = lib.func('size_t zke_agg_bytes(size_t)');
 const zke_aggregate = lib.func('int64_t zke_aggregate(void*, const char*, size_t, const uint8_t*, const uint8_t*, uint8_t*, size_t, char*, size_t)');
 const zke_agg_verify = lib.func('int zke_agg_verify(const char*, const char*, size_t, const uint8_t*, const uint8_t*, size_t, char*, size_t)');
 
+const zke_poseidon_hash = lib.func('int zke_poseidon_hash(const uint8_t*, size_t, uint8_t*)');
+
 const cstr = (b: Buffer) => b.toString('utf8', 0, b.indexOf(0));
 type Entry = { circuit: unknown; zkey: unknown; ctx: unknown };
 const registry = new Map<string, Entry>();
@@ -132,3 +134,29 @@ export const aggregation = {
     return rc === 1;
   },
 };
+
+/** Poseidon hashes of packages/helpers/src/hash.ts on the library's host permutation (zke_poseidon_hash), synchronous:
+ *  what a hashed (`"reveal": "hash"`) or committed (`"reveal": "commit"`) app output holds. */
+const R = 21888242871839275222246405745257275088548364400416034343698204186575808495617n;
+const le32 = (x: bigint) => { const b = Buffer.alloc(32); let v = ((x % R) + R) % R; for (let i = 0; i < 32; i++) { b[i] = Number(v & 0xffn); v >>= 8n; } return b; };
+export function poseidon(inputs: bigint[]): bigint {
+  if (inputs.length < 1 || inputs.length > 16) throw new Error(`Poseidon takes 1 to 16 inputs, not ${inputs.length}`);
+  const out = Buffer.alloc(32);
+  if (zke_poseidon_hash(Buffer.concat(inputs.map(le32)), inputs.length, out) !== 0) throw new Error('zke_poseidon_hash failed');
+  let v = 0n;
+  for (let i = 31; i >= 0; i--) v = (v << 8n) | BigInt(out[i]);
+  return v;
+}
+export function poseidonLarge(input: bigint, numChunks: number, bitsPerChunk: number): bigint {
+  const mask = (1n << BigInt(bitsPerChunk)) - 1n;
+  return poseidon(Array.from({ length: numChunks }, (_, i) => (input >> BigInt(i * bitsPerChunk)) & mask));
+}
+export function poseidonModular(inputs: bigint[]): bigint {
+  let out: bigint | null = null;
+  for (let start = 0; start < inputs.length; start += 16) {
+    const h = poseidon(inputs.slice(start, start + 16));
+    out = out === null ? h : poseidon([out, h]);
+  }
+  if (out === null) throw new Error('No inputs provided');
+  return out;
+}
