@@ -57,9 +57,13 @@ zke_circuit* zke_circuit_build_regex(const char* const* parts, const uint8_t* is
  * location: "header" | "body", parts: [{regexDef, isPublic, maxLength}]}) a regex that must match and, per public part, a
  * PackRegexReveal output (`name`, or `name0`, `name1`, ... for several public parts) with its private index input
  * (`nameIndex` / `name0Index`, ...); `externalInputs` ([{name, maxLength?}]) are public inputs, one field element or
- * ceil(maxLength / 31) packed ones; `emailNullifier` adds the EmailNullifier output.  Signal order: outputs (pubkeyHash,
- * shaHi, shaLo, masks, regex outputs, emailNullifier), public inputs (external inputs, pubkey if public), the
- * EmailVerifier inputs, then the index inputs.  A malformed spec is refused with a message naming the field. */
+ * ceil(maxLength / 31) packed ones; `emailNullifier` adds the EmailNullifier output.  `keyRegistryDepth` d (1..32; 0 or
+ * absent: no registry) hides the signing key: pubkeyHash stays private and is proven a leaf of a Poseidon(2) Merkle tree
+ * of depth d (zke_merkle_build), whose root `registryRoot` is published in pubkeyHash's place; the private inputs
+ * registryIndex and registrySiblings[d] come last.  It is refused with publicPubkey, and the three names are then
+ * reserved.  Signal order: outputs (pubkeyHash or registryRoot, shaHi, shaLo, masks, regex outputs, emailNullifier),
+ * public inputs (external inputs, pubkey if public), the EmailVerifier inputs, the index inputs, private external inputs,
+ * then registryIndex and registrySiblings.  A malformed spec is refused with a message naming the field. */
 zke_circuit* zke_circuit_build_app(const char* spec_json, char* err, size_t errcap);
 void zke_circuit_free(zke_circuit* c);
 /* circom's constraint system: an iden3 `.r1cs` image (what `circom --r1cs` writes and `snarkjs r1cs info` / `snarkjs groth16
@@ -157,6 +161,26 @@ int zke_circuit_program_stats_ex(const zke_circuit* c, uint32_t flags, uint32_t 
  * permutation the circuits constrain (the `poseidon` of @zk-email/helpers).  Returns 0, -1 for a bad n or pointer, -2 for an
  * input not below r. */
 int zke_poseidon_hash(const uint8_t* inputs, size_t n, uint8_t* out);
+
+/* Merkle registry of DKIM keys, on the GPU (registry.cu).  Field elements are 32-byte little-endian.  Without a device
+ * these return the library's "no CUDA device available (this library has no CPU fallback)" error; argument refusals
+ * come first.  Each returns < 0 with a message in err on a refusal.
+ * zke_poseidon_batch: out[count][32] = Poseidon(width)(inputs[i][0..width-1]) for width 1..16, the values of
+ *   zke_poseidon_hash; an input not below r is refused, naming its instance.  Returns 0.
+ * zke_pubkey_hashes: the pubkeyHash of each of `count` RSA moduli (modulus_bytes each, little-endian): k limbs of n
+ *   bits, merged in pairs as PoseidonLarge does, through Poseidon(ceil(k / 2)).  Refuses k outside 17..32, 2n >= 251
+ *   and a modulus >= 2^(n k).  Returns 0.
+ * zke_merkle_build: every level of the tree of depth 1..32 over count <= 2^depth leaves (below r), node hash
+ *   H(l, r) = Poseidon(2)([l, r]).  Level l holds ceil(count / 2^l) nodes, a missing right child at level l is
+ *   zeros[l] (zeros[0] = 0, zeros[l + 1] = H(zeros[l], zeros[l])); levels are written one after the other from the
+ *   leaves (level 0) to the root.  Returns the bytes written, the size needed when levels == NULL, -2 if cap is too small.
+ * zke_registry_device_ms: device time of the calling thread's last successful call above (CUDA events around its kernels). */
+int zke_poseidon_batch(const uint8_t* inputs, uint32_t width, size_t count, int device, uint8_t* out, char* err, size_t errcap);
+int zke_pubkey_hashes(const uint8_t* moduli, size_t count, uint32_t modulus_bytes, uint32_t n, uint32_t k, int device,
+                      uint8_t* out, char* err, size_t errcap);
+int64_t zke_merkle_build(const uint8_t* leaves, size_t count, uint32_t depth, int device, uint8_t* levels, size_t cap,
+                         char* err, size_t errcap);
+double zke_registry_device_ms(void);
 
 
 /* ---------------------------------------------------------------------------------------------------

@@ -210,6 +210,13 @@ Circuit build_named(const std::string& name, const std::vector<int64_t>& p) {
         auto out = b.declare_outputs("out", 1);
         LCVec in = inputs(b, "in", (uint32_t)p[0]);
         outputs(b, "out", {poseidon_modular(b, in)}, out);
+    } else if (name == "BinaryMerkleRoot") {
+        need(1);
+        if (p[0] < 1 || p[0] > 32) throw std::runtime_error("BinaryMerkleRoot: depth must be 1..32");
+        auto out = b.declare_outputs("root", 1);
+        LC leaf = inputs(b, "leaf", 1)[0], index = inputs(b, "index", 1)[0];
+        LCVec sib = inputs(b, "siblings", (uint32_t)p[0]);
+        outputs(b, "root", {binary_merkle_root(b, leaf, index, sib)}, out);
     } else if (name == "RemoveSoftLineBreaks") {   // test-circuits/remove-soft-line-breaks-test.circom
         need(1);
         auto out = b.declare_outputs("isValid", 1);

@@ -215,7 +215,7 @@ const uint32_t MAX_EXTERNAL_BYTES = 1u << 16;
 gadgets::AppSpec app_spec_of(const JV& s) {
     only_keys(s, "spec", {"maxHeadersLength", "maxBodyLength", "n", "k", "ignoreBodyHashCheck", "enableHeaderMasking",
                           "enableBodyMasking", "removeSoftLineBreaks", "publicPubkey", "regexStyle", "exposeHeaderHash",
-                          "regexes", "externalInputs", "emailNullifier", "shaPrecomputeSelector"});
+                          "regexes", "externalInputs", "emailNullifier", "shaPrecomputeSelector", "keyRegistryDepth"});
     gadgets::AppSpec a;
     gadgets::EmailVerifierParams& ev = a.ev;
     if (const JV* v = s.get("maxHeadersLength")) ev.max_headers_length = uint_of(*v, "maxHeadersLength");
@@ -238,6 +238,10 @@ gadgets::AppSpec app_spec_of(const JV& s) {
         if (v->type != JV::STR && v->type != JV::NUL) throw std::runtime_error("shaPrecomputeSelector: expected a string");
     a.expose_header_hash = bool_of(s, "exposeHeaderHash", true, "");
     a.email_nullifier = bool_of(s, "emailNullifier", false, "");
+    if (const JV* v = s.get("keyRegistryDepth")) {
+        a.key_registry_depth = uint_of(*v, "keyRegistryDepth");
+        if (a.key_registry_depth > 32) throw std::runtime_error("keyRegistryDepth: at most 32, not " + v->s);
+    }
     if (const JV* rs = array_of(s, "regexes")) {
         for (size_t r = 0; r < rs->arr.size(); ++r) {
             const JV& e = rs->arr[r];

@@ -14,6 +14,7 @@ cudaError_t upload_constants_msm_g1(const FieldConsts*, const FieldConsts*);
 cudaError_t upload_constants_msm_g2(const FieldConsts*, const FieldConsts*);
 cudaError_t upload_constants_fixed_base(const FieldConsts*, const FieldConsts*);
 cudaError_t upload_constants_verify(const FieldConsts*, const FieldConsts*);
+cudaError_t upload_constants_registry(const FieldConsts*, const FieldConsts*);
 } }
 
 #include "../../include/zkemail_b200.h"
@@ -47,6 +48,7 @@ void zke::select_device(int device) {
     CUDA_OK(dev::upload_constants_msm_g2(&fr, &fq));
     CUDA_OK(dev::upload_constants_fixed_base(&fr, &fq));
     CUDA_OK(dev::upload_constants_verify(&fr, &fq));
+    CUDA_OK(dev::upload_constants_registry(&fr, &fq));
     CUDA_OK(dev::configure_witness_kernel());   // per-device function attribute (> 48 KB dynamic shared memory)
 }
 

@@ -843,6 +843,22 @@ LC poseidon_modular(Builder& b, const LCVec& in, bool record) {
     return out;
 }
 
+// ---------------------------------------------------------------- Merkle registry of keys
+LC binary_merkle_root(Builder& b, const LC& leaf, const LC& index, const LCVec& siblings) {
+    ScopeGuard g(b, "BinaryMerkleRoot");
+    const uint32_t depth = (uint32_t)siblings.size();
+    if (depth < 1 || depth > 32) throw std::runtime_error("BinaryMerkleRoot: depth must be 1..32");
+    LCVec bits = num2bits(b, index, depth);
+    const bool record = b.materialize_linear;           // a record needs its inputs as signals
+    LC cur = leaf;
+    for (uint32_t l = 0; l < depth; ++l) {
+        LC d = b.mul(bits[l], siblings[l] - cur);       // bit = 1: swap, the node is a right child
+        LC left = b.signal(cur + d), right = b.signal(siblings[l] - d);
+        cur = poseidon(b, {left, right}, record);
+    }
+    return cur;
+}
+
 // ---------------------------------------------------------------- helpers/remove-soft-line-breaks.circom
 LC remove_soft_line_breaks(Builder& b, const LCVec& encoded, const LCVec& decoded) {
     ScopeGuard g(b, "RemoveSoftLineBreaks");
@@ -982,13 +998,27 @@ Circuit build_email_app(const AppSpec& A, bool materialize_linear) {
     }
     for (size_t e = 0; e < A.external_inputs.size(); ++e) claim("externalInputs[" + std::to_string(e) + "].name", A.external_inputs[e].name);
 
+    // the key registry: registryRoot replaces pubkeyHash as the first output, its inputs take the three names
+    const uint32_t depth = A.key_registry_depth;
+    if (depth > 32) throw std::runtime_error("keyRegistryDepth: at most 32, not " + std::to_string(depth));
+    if (depth && P.public_pubkey)
+        throw std::runtime_error("keyRegistryDepth: publicPubkey publishes the key the registry hides; drop one of them");
+    static const char* const REGISTRY_SIGNALS[] = {"registryRoot", "registryIndex", "registrySiblings"};
+    auto check_registry = [&](const std::string& field, const std::string& name) {
+        for (const char* r : REGISTRY_SIGNALS)
+            if (depth && name == r) throw std::runtime_error(field + ": signal name '" + name + "' is taken by the key registry (keyRegistryDepth)");
+    };
+    for (size_t r = 0; r < A.regexes.size(); ++r)
+        for (auto& rv : reveals[r]) { check_registry("regexes[" + std::to_string(r) + "].name", rv.out); check_registry("regexes[" + std::to_string(r) + "].name", rv.index); }
+    for (size_t e = 0; e < A.external_inputs.size(); ++e) check_registry("externalInputs[" + std::to_string(e) + "].name", A.external_inputs[e].name);
+
     Builder b("EmailVerifier");
     b.materialize_linear = materialize_linear;
     if (P.regex_style >= 0) b.regex_style = P.regex_style;
     ScopeGuard g(b, "EmailVerifier");
 
     // outputs first (circom witness order)
-    Var pubkey_hash = b.declare_outputs("pubkeyHash", 1)[0];
+    Var pubkey_hash = b.declare_outputs(depth ? "registryRoot" : "pubkeyHash", 1)[0];
     Var sha_hi = 0, sha_lo = 0;
     if (A.expose_header_hash) { sha_hi = b.declare_outputs("shaHi", 1)[0]; sha_lo = b.declare_outputs("shaLo", 1)[0]; }
     std::vector<Var> masked_header, masked_body;
@@ -1030,6 +1060,12 @@ Circuit build_email_app(const AppSpec& A, bool materialize_linear) {
     for (size_t e = 0; e < A.external_inputs.size(); ++e) {     // private external inputs: after everything else
         const AppExternalInput& ei = A.external_inputs[e];
         if (!ei.is_public) external_first[e] = b.declare_inputs(ei.name, ei.max_length ? packed_len(ei.max_length) : 1, false)[0];
+    }
+    LC registry_index;
+    LCVec registry_siblings;
+    if (depth) {
+        registry_index = LC(b.declare_inputs("registryIndex", 1, false)[0]);
+        registry_siblings = to_lcs(b.declare_inputs("registrySiblings", depth, false));
     }
 
     num2bits(b, email_header_length, log2_ceil(H));                      // :58-59
@@ -1079,7 +1115,9 @@ Circuit build_email_app(const AppSpec& A, bool materialize_linear) {
             for (uint32_t i = 0; i < Bd; ++i) b.assign_output(masked_body[i], m[i]);
         }
     }
-    b.assign_output(pubkey_hash, poseidon_large(b, n, pubkey));          // :173
+    LC key_hash = poseidon_large(b, n, pubkey);                          // :173
+    if (depth) key_hash = binary_merkle_root(b, key_hash, registry_index, registry_siblings);
+    b.assign_output(pubkey_hash, key_hash);
     if (A.regexes.empty() && !A.email_nullifier) return b.finalize();
 
     ScopeGuard ag(b, A.scope);

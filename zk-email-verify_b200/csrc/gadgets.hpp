@@ -61,6 +61,9 @@ LCVec select_regex_reveal(Builder& b, const LCVec& in, const LC& start_index, ui
 LC poseidon_large(Builder& b, uint32_t bits_per_chunk, const LCVec& in);    // utils/hash.circom:15-39
 LC poseidon_modular(Builder& b, const LCVec& in, bool record = false);      // utils/hash.circom:49-83
 LC remove_soft_line_breaks(Builder& b, const LCVec& encoded, const LCVec& decoded);   // helpers/remove-soft-line-breaks.circom:14-126 (returns isValid)
+// root of a binary Poseidon(2) Merkle tree of depth siblings.size() (1..32) from a leaf, its index (bit l set: the node at
+// level l is a right child; index < 2^depth is enforced) and the authentication path; each node hash is recorded
+LC binary_merkle_root(Builder& b, const LC& leaf, const LC& index, const LCVec& siblings);
 
 // ---- lib/ ------------------------------------------------------------------------------------
 LCVec sha256_general(Builder& b, const LCVec& padded_in_bits, const LC& padded_in_length_bits,
@@ -138,6 +141,9 @@ struct AppSpec {
     std::vector<AppExternalInput> external_inputs;
     bool email_nullifier = false;
     std::string scope = "EmailApp";    // scope of everything after pubkeyHash
+    // 1..32: pubkeyHash stays private and is proven a leaf of a Merkle registry of keys; the output registryRoot takes
+    // its place, the private inputs registryIndex and registrySiblings[depth] come last.  0: no registry
+    uint32_t key_registry_depth = 0;
 };
 Circuit build_email_app(const AppSpec& spec, bool materialize_linear = true);
 

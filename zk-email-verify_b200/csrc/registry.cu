@@ -1,0 +1,405 @@
+// Batched Poseidon and the Merkle registry of DKIM keys (include/zkemail_b200.h: zke_poseidon_batch, zke_pubkey_hashes,
+// zke_merkle_build).
+//
+// One thread runs one Poseidon instance: the Merkle node hash (width 3) with its state in registers, the other widths
+// from one instantiation that takes the width at run time (its state in the thread's stack frame).  The round constants and the MDS matrix of the width come from
+// gadgets::poseidon_params - the tables the circuits constrain and the witness kernel's native op reads - and every
+// block stages them in shared memory in Montgomery form.  The permutation is circomlib's plain schedule: full rounds
+// S-box every lane, partial rounds lane 0 only, a dense t x t mix after each round.
+//
+// The Merkle tree (node H(l, r) = Poseidon(2)([l, r])) is built level by level on the device: one kernel hashes the
+// lowest FUSE_LEVELS levels of a 2^FUSE_LEVELS-leaf subtree per block, keeping each level in shared memory, and one launch
+// per higher level hashes the pairs of the level below.  A missing right child at level l is zeros[l], the root of an
+// empty subtree of height l (computed on the host: at most 32 hashes).
+#include "ff.cuh"
+#include "device_engine.cuh"
+#include "cuda_host.hpp"
+#include "gadgets.hpp"
+#include "../../include/zkemail_b200.h"
+#include <cstring>
+#include <stdexcept>
+#include <string>
+#include <vector>
+
+namespace zke {
+void set_err(char* err, size_t cap, const std::string& msg);   // capi_circuit.cpp
+}
+
+namespace zke {
+namespace dev {
+
+ZKE_DEFINE_CONSTANT_UPLOAD(upload_constants_registry)
+
+static const int REG_THREADS = 128;
+static const int FUSE_LEVELS = 8;                 // levels 1..8 of a 256-leaf subtree per block of 128 threads
+static const uint32_t NO_BAD = 0xffffffffu;
+
+// Montgomery form from 8 little-endian standard-form words; *bad is set when the value is not below r
+__device__ __forceinline__ Fr fr_in(const uint32_t w[8], bool* bad) {
+    Fr x;
+    for (int i = 0; i < 8; ++i) x.v[i] = w[i];
+    if (!below_modulus(x)) *bad = true;
+    return x.to_mont();
+}
+__device__ __forceinline__ Fr fr_load(const uint8_t* p, bool* bad) {
+    uint32_t w[8];
+    const uint4* q = reinterpret_cast<const uint4*>(p);
+    const uint4 a = q[0], b = q[1];
+    w[0] = a.x; w[1] = a.y; w[2] = a.z; w[3] = a.w; w[4] = b.x; w[5] = b.y; w[6] = b.z; w[7] = b.w;
+    return fr_in(w, bad);
+}
+__device__ __forceinline__ void fr_store(uint8_t* p, const Fr& x) { x.from_mont().store(p); }
+
+// constants of width T: rc[(R_F + R_P) * T] then mds[T][T], standard form in global memory -> Montgomery in shared memory
+__device__ __forceinline__ void stage_constants(Fr* sh, const uint8_t* g, uint32_t n) {
+    for (uint32_t i = threadIdx.x; i < n; i += blockDim.x) sh[i] = Fr::load(g + 32ull * i).to_mont();
+    __syncthreads();
+}
+
+__device__ __forceinline__ Fr sbox(const Fr& x) { Fr x2 = x.sqr(); Fr x4 = x2.sqr(); return x4 * x; }
+
+// circomlib Poseidon(t - 1) of st[1..t-1] (st[0] = 0 on entry); returns the output state[0].  T > 0: the width is a
+// compile-time constant and the state lives in registers (the Merkle node hash, T = 3); T = 0: any width t <= MAX_T
+// from one instantiation (unrolling the dense mix for all sixteen widths takes nvcc tens of minutes)
+static const int MAX_T = 17;
+template <int T>
+__device__ __forceinline__ Fr permute(Fr* st, int t, const Fr* rc, const Fr* mds, int r_p) {
+    if (T > 0) t = T;
+    const int rounds = 8 + r_p;
+    Fr nx[T > 0 ? T : MAX_T];
+#pragma unroll 1
+    for (int rnd = 0; rnd < rounds; ++rnd) {
+        const Fr* c = rc + rnd * t;
+#pragma unroll
+        for (int i = 0; i < (T > 0 ? T : t); ++i) st[i] = st[i] + c[i];
+        if (rnd < 4 || rnd >= 4 + r_p) {
+#pragma unroll
+            for (int i = 0; i < (T > 0 ? T : t); ++i) st[i] = sbox(st[i]);
+        } else {
+            st[0] = sbox(st[0]);
+        }
+#pragma unroll
+        for (int i = 0; i < (T > 0 ? T : t); ++i) {
+            Fr acc = mds[i * t] * st[0];
+#pragma unroll
+            for (int j = 1; j < (T > 0 ? T : t); ++j) acc = acc + mds[i * t + j] * st[j];
+            nx[i] = acc;
+        }
+#pragma unroll
+        for (int i = 0; i < (T > 0 ? T : t); ++i) st[i] = nx[i];
+    }
+    return st[0];
+}
+
+__device__ __forceinline__ uint32_t n_constants(int t, int r_p) { return (uint32_t)((8 + r_p) * t + t * t); }
+
+// out[i] = Poseidon(t - 1)(in[i][0..t-2]); the first instance holding an input not below r goes to *bad
+__global__ void __launch_bounds__(REG_THREADS)
+poseidon_batch_kernel(const uint8_t* __restrict__ in, uint64_t count, int t, const uint8_t* __restrict__ consts, int r_p,
+                      uint8_t* __restrict__ out, uint32_t* __restrict__ bad) {
+    extern __shared__ uint4 smem[];
+    Fr* sh = reinterpret_cast<Fr*>(smem);
+    stage_constants(sh, consts, n_constants(t, r_p));
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= count) return;
+    bool b = false;
+    Fr st[MAX_T];
+    st[0] = Fr::zero();
+#pragma unroll 1
+    for (int k = 1; k < t; ++k) st[k] = fr_load(in + 32ull * ((uint64_t)(t - 1) * i + (k - 1)), &b);
+    if (b) atomicMin(bad, (uint32_t)min(i, (uint64_t)NO_BAD - 1));
+    fr_store(out + 32ull * i, permute<0>(st, t, sh, sh + (8 + r_p) * t, r_p));
+}
+
+// bits [off, off + w) of a little-endian byte string of `len` bytes (bits past the end read as 0), w <= 256
+__device__ __forceinline__ void bit_field(const uint8_t* m, uint32_t len, uint32_t off, uint32_t w, uint32_t out[8]) {
+    for (int q = 0; q < 8; ++q) {
+        const uint32_t lo = 32 * q;
+        if (lo >= w) { out[q] = 0; continue; }
+        const uint32_t pos = off + lo, byte = pos >> 3;
+        uint64_t v = 0;
+        for (int k = 0; k < 5; ++k) if (byte + k < len) v |= (uint64_t)m[byte + k] << (8 * k);
+        uint32_t x = (uint32_t)(v >> (pos & 7));
+        const uint32_t keep = w - lo;
+        if (keep < 32) x &= (1u << keep) - 1;
+        out[q] = x;
+    }
+}
+
+// PoseidonLarge leaves: modulus i (mlen bytes, little-endian) -> its k limbs of n bits, merged in pairs (limb 2j + limb
+// 2j+1 * 2^n, the last limb alone for odd k) = the 2n-bit chunks of the modulus, hashed with Poseidon(T - 1), T - 1 =
+// ceil(k / 2).  A modulus with a bit at or above n k goes to *bad.
+__global__ void __launch_bounds__(REG_THREADS)
+pubkey_hash_kernel(const uint8_t* __restrict__ moduli, uint64_t count, uint32_t mlen, uint32_t n, uint32_t k,
+                   const uint8_t* __restrict__ consts, int r_p, uint8_t* __restrict__ out, uint32_t* __restrict__ bad) {
+    extern __shared__ uint4 smem[];
+    Fr* sh = reinterpret_cast<Fr*>(smem);
+    const int t = (int)(k + 1) / 2 + 1;
+    stage_constants(sh, consts, n_constants(t, r_p));
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= count) return;
+    const uint8_t* m = moduli + (uint64_t)mlen * i;
+    const uint32_t nk = n * k;
+    bool b = false;
+    for (uint32_t byte = nk >> 3; byte < mlen; ++byte) {
+        const uint32_t first = byte == (nk >> 3) ? (nk & 7) : 0;
+        if (m[byte] >> first) b = true;
+    }
+    Fr st[MAX_T];
+    st[0] = Fr::zero();
+#pragma unroll 1
+    for (int j = 1; j < t; ++j) {
+        const uint32_t off = 2 * n * (j - 1);
+        uint32_t w[8];
+        bit_field(m, mlen, off, min(2 * n, nk - off), w);
+        st[j] = fr_in(w, &b);
+    }
+    if (b) atomicMin(bad, (uint32_t)min(i, (uint64_t)NO_BAD - 1));
+    fr_store(out + 32ull * i, permute<0>(st, t, sh, sh + (8 + r_p) * t, r_p));
+}
+
+__device__ __forceinline__ Fr node_hash(const Fr& l, const Fr& r, const Fr* rc, const Fr* mds, int r_p) {
+    Fr st[3] = {Fr::zero(), l, r};
+    return permute<3>(st, 3, rc, mds, r_p);
+}
+
+// Levels 1..L of the tree (L <= FUSE_LEVELS): block b owns the nodes under its 2^L leaves.  levels: the whole level
+// image, level l starting at off[l] with size[l] nodes (level 0 = the leaves, uploaded); zeros[l] standard form.
+struct LevelTable { uint64_t off[33], size[33]; };
+
+__global__ void __launch_bounds__(REG_THREADS)
+merkle_fused_kernel(uint8_t* __restrict__ levels, LevelTable lt, int L, const uint8_t* __restrict__ consts, int r_p,
+                    const uint8_t* __restrict__ zeros, uint32_t* __restrict__ bad) {
+    extern __shared__ uint4 smem[];
+    Fr* sh = reinterpret_cast<Fr*>(smem);
+    const uint32_t nc = n_constants(3, r_p);
+    Fr* node = sh + nc;                                   // [REG_THREADS] nodes of the level just built
+    stage_constants(sh, consts, nc);
+    const Fr* rc = sh;
+    const Fr* mds = sh + (8 + r_p) * 3;
+    const uint32_t t = threadIdx.x;
+    bool b = false;
+    for (int l = 1; l <= L; ++l) {
+        const uint32_t width = 1u << (L - l);             // nodes of level l under this block
+        const uint64_t j = (uint64_t)blockIdx.x * width + t;
+        Fr h;
+        const bool live = t < width && j < lt.size[l];
+        if (live) {
+            Fr left, right;
+            const bool has_right = 2 * j + 1 < lt.size[l - 1];
+            if (l == 1) {
+                left = fr_load(levels + 32 * (lt.off[0] + 2 * j), &b);
+                right = has_right ? fr_load(levels + 32 * (lt.off[0] + 2 * j + 1), &b) : Fr::zero();
+            } else {
+                left = node[2 * t];
+                right = has_right ? node[2 * t + 1] : fr_load(zeros + 32 * (l - 1), &b);
+            }
+            h = node_hash(left, right, rc, mds, r_p);
+            fr_store(levels + 32 * (lt.off[l] + j), h);
+        }
+        __syncthreads();                                  // every read of the level below is done
+        if (live) node[t] = h;
+        __syncthreads();
+    }
+    if (b) atomicMin(bad, (uint32_t)min((uint64_t)blockIdx.x << FUSE_LEVELS, (uint64_t)NO_BAD - 1));
+}
+
+// level l > FUSE_LEVELS from level l - 1 in global memory
+__global__ void __launch_bounds__(REG_THREADS)
+merkle_level_kernel(uint8_t* __restrict__ levels, uint64_t below_off, uint64_t below_size, uint64_t off, uint64_t size,
+                    const uint8_t* __restrict__ consts, int r_p, const uint8_t* __restrict__ zero_below) {
+    extern __shared__ uint4 smem[];
+    Fr* sh = reinterpret_cast<Fr*>(smem);
+    stage_constants(sh, consts, n_constants(3, r_p));
+    const uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= size) return;
+    bool b = false;
+    const Fr left = fr_load(levels + 32 * (below_off + 2 * j), &b);
+    const Fr right = fr_load(2 * j + 1 < below_size ? levels + 32 * (below_off + 2 * j + 1) : zero_below, &b);
+    fr_store(levels + 32 * (off + j), node_hash(left, right, sh, sh + (8 + r_p) * 3, r_p));
+}
+
+}  // namespace dev
+}  // namespace zke
+
+using namespace zke;
+
+namespace {
+
+thread_local double g_last_device_ms = 0;     // zke_registry_device_ms
+
+// rc then mds of Poseidon width t, standard form, on the device
+struct WidthConsts {
+    DevBuf buf;
+    int r_p = 0;
+    uint32_t n = 0;
+    explicit WidthConsts(int t) {
+        const gadgets::PoseidonParams& P = gadgets::poseidon_params(t);
+        std::vector<U256> v;
+        for (const Fr& c : P.rc) v.push_back(c.to_u256());
+        for (int i = 0; i < t; ++i) for (int j = 0; j < t; ++j) v.push_back(P.mds[i][j].to_u256());
+        r_p = P.r_p;
+        n = (uint32_t)v.size();
+        buf.upload(v);
+    }
+    size_t smem() const { return 32ull * n; }
+};
+
+struct Timer {
+    cudaEvent_t a = nullptr, b = nullptr;
+    Timer() { CUDA_OK(cudaEventCreate(&a)); CUDA_OK(cudaEventCreate(&b)); CUDA_OK(cudaEventRecord(a)); }
+    ~Timer() { if (a) cudaEventDestroy(a); if (b) cudaEventDestroy(b); }
+    void stop() {          // after the last kernel: the device time of the call's kernels
+        CUDA_OK(cudaEventRecord(b));
+        CUDA_OK(cudaEventSynchronize(b));
+        float ms = 0;
+        CUDA_OK(cudaEventElapsedTime(&ms, a, b));
+        g_last_device_ms = ms;
+    }
+};
+
+uint32_t read_bad(const DevBuf& bad) {
+    uint32_t v = 0;
+    CUDA_OK(cudaMemcpy(&v, bad.p, 4, cudaMemcpyDeviceToHost));
+    return v;
+}
+
+void bad_flag(DevBuf& d) {
+    d.alloc(4);
+    CUDA_OK(cudaMemset(d.p, 0xff, 4));
+}
+
+uint32_t blocks_for(uint64_t count) {
+    const uint64_t b = (count + dev::REG_THREADS - 1) / dev::REG_THREADS;
+    if (b > 0x7fffffffull) throw std::runtime_error("count too large");
+    return (uint32_t)b;
+}
+
+template <class K>
+void set_smem(K kernel, size_t bytes) {
+    CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+}
+
+}  // namespace
+
+extern "C" {
+
+int zke_poseidon_batch(const uint8_t* inputs, uint32_t width, size_t count, int device, uint8_t* out, char* err, size_t errcap) {
+    try {
+        if (!inputs || !out) throw std::runtime_error("null argument");
+        if (width < 1 || width > 16) throw std::runtime_error("width must be 1..16, not " + std::to_string(width));
+        if (count == 0) return 0;
+        select_device(device);
+        const int t = (int)width + 1;
+        WidthConsts C(t);
+        DevBuf din, dout, bad;
+        bad_flag(bad);
+        din.alloc(32ull * width * count);
+        dout.alloc(32ull * count);
+        CUDA_OK(cudaMemcpy(din.p, inputs, din.bytes, cudaMemcpyHostToDevice));
+        Timer tm;
+        set_smem(dev::poseidon_batch_kernel, C.smem());
+        dev::poseidon_batch_kernel<<<blocks_for(count), dev::REG_THREADS, C.smem()>>>(din.p, count, t, C.buf.p, C.r_p, dout.p,
+                                                                                     reinterpret_cast<uint32_t*>(bad.p));
+        ZKE_COUNT_LAUNCH(1);
+        CHECK_LAUNCH();
+        tm.stop();
+        const uint32_t b = read_bad(bad);
+        if (b != dev::NO_BAD) throw std::runtime_error("instance " + std::to_string(b) + ": an input is not below r");
+        CUDA_OK(cudaMemcpy(out, dout.p, dout.bytes, cudaMemcpyDeviceToHost));
+        return 0;
+    } catch (const std::exception& e) { set_err(err, errcap, e.what()); return -1; }
+}
+
+int zke_pubkey_hashes(const uint8_t* moduli, size_t count, uint32_t modulus_bytes, uint32_t n, uint32_t k, int device,
+                      uint8_t* out, char* err, size_t errcap) {
+    try {
+        if (!moduli || !out) throw std::runtime_error("null argument");
+        if (k < 17 || k > 32) throw std::runtime_error("k must be 17..32 (PoseidonLarge), not " + std::to_string(k));
+        if (n == 0 || 2 * n >= 251) throw std::runtime_error("n must satisfy 0 < 2n < 251 (PoseidonLarge), not " + std::to_string(n));
+        if (modulus_bytes == 0) throw std::runtime_error("modulus_bytes must be positive");
+        if (count == 0) return 0;
+        select_device(device);
+        const int t = (int)(k + 1) / 2 + 1;
+        WidthConsts C(t);
+        DevBuf dm, dout, bad;
+        bad_flag(bad);
+        dm.alloc((size_t)modulus_bytes * count);
+        dout.alloc(32ull * count);
+        CUDA_OK(cudaMemcpy(dm.p, moduli, dm.bytes, cudaMemcpyHostToDevice));
+        Timer tm;
+        set_smem(dev::pubkey_hash_kernel, C.smem());
+        dev::pubkey_hash_kernel<<<blocks_for(count), dev::REG_THREADS, C.smem()>>>(dm.p, count, modulus_bytes, n, k, C.buf.p, C.r_p,
+                                                                                  dout.p, reinterpret_cast<uint32_t*>(bad.p));
+        ZKE_COUNT_LAUNCH(1);
+        CHECK_LAUNCH();
+        tm.stop();
+        const uint32_t b = read_bad(bad);
+        if (b != dev::NO_BAD)
+            throw std::runtime_error("modulus " + std::to_string(b) + " is not below 2^(n k) = 2^" + std::to_string(n * k));
+        CUDA_OK(cudaMemcpy(out, dout.p, dout.bytes, cudaMemcpyDeviceToHost));
+        return 0;
+    } catch (const std::exception& e) { set_err(err, errcap, e.what()); return -1; }
+}
+
+int64_t zke_merkle_build(const uint8_t* leaves, size_t count, uint32_t depth, int device, uint8_t* levels, size_t cap,
+                         char* err, size_t errcap) {
+    try {
+        if (!leaves) throw std::runtime_error("null argument");
+        if (depth < 1 || depth > 32) throw std::runtime_error("depth must be 1..32, not " + std::to_string(depth));
+        if (count == 0) throw std::runtime_error("count must be at least 1");
+        if ((uint64_t)count > (1ull << depth))
+            throw std::runtime_error("count " + std::to_string(count) + " does not fit a tree of depth " + std::to_string(depth));
+        dev::LevelTable lt;
+        uint64_t total = 0;
+        for (uint32_t l = 0; l <= depth; ++l) {
+            lt.off[l] = total;
+            lt.size[l] = (count + (1ull << l) - 1) >> l;
+            total += lt.size[l];
+        }
+        const int64_t bytes = (int64_t)(32 * total);
+        if (!levels) return bytes;
+        if (cap < (size_t)bytes) return -2;
+        select_device(device);
+        std::vector<U256> zeros(depth + 1);
+        zeros[0] = U256{{0, 0, 0, 0}};
+        Fr z = Fr::zero();
+        for (uint32_t l = 1; l <= depth; ++l) { z = gadgets::poseidon_hash({z, z}); zeros[l] = z.to_u256(); }
+        WidthConsts C(3);
+        DevBuf d, dz, bad;
+        bad_flag(bad);
+        dz.upload(zeros);
+        d.alloc((size_t)bytes);
+        CUDA_OK(cudaMemcpy(d.p, leaves, 32ull * count, cudaMemcpyHostToDevice));
+        const int L = depth < (uint32_t)dev::FUSE_LEVELS ? (int)depth : dev::FUSE_LEVELS;
+        const size_t smem = C.smem(), smem_fused = smem + 32ull * dev::REG_THREADS;
+        set_smem(dev::merkle_fused_kernel, smem_fused);
+        Timer tm;
+        dev::merkle_fused_kernel<<<(uint32_t)((count + (1ull << L) - 1) >> L), dev::REG_THREADS, smem_fused>>>(d.p, lt, L, C.buf.p, C.r_p, dz.p, reinterpret_cast<uint32_t*>(bad.p));
+        ZKE_COUNT_LAUNCH(1);
+        CHECK_LAUNCH();
+        for (uint32_t l = (uint32_t)L + 1; l <= depth; ++l) {
+            dev::merkle_level_kernel<<<blocks_for(lt.size[l]), dev::REG_THREADS, smem>>>(d.p, lt.off[l - 1], lt.size[l - 1], lt.off[l],
+                                                                                       lt.size[l], C.buf.p, C.r_p, dz.p + 32ull * (l - 1));
+            ZKE_COUNT_LAUNCH(1);
+            CHECK_LAUNCH();
+        }
+        tm.stop();
+        const uint32_t b = read_bad(bad);
+        if (b != dev::NO_BAD) {
+            // the fused kernel reports the first leaf of the block: find the leaf on the host
+            for (uint64_t i = b; i < count; ++i) {
+                U256 x;
+                memcpy(x.v, leaves + 32 * i, 32);
+                if (u256_cmp(x, fr_params().p) >= 0) throw std::runtime_error("leaf " + std::to_string(i) + " is not below r");
+            }
+            throw std::runtime_error("a leaf is not below r");
+        }
+        CUDA_OK(cudaMemcpy(levels, d.p, (size_t)bytes, cudaMemcpyDeviceToHost));
+        return bytes;
+    } catch (const std::exception& e) { set_err(err, errcap, e.what()); return -1; }
+}
+
+double zke_registry_device_ms(void) { return g_last_device_ms; }
+
+}  // extern "C"

@@ -11,6 +11,7 @@ from .input_generators import (generate_circuit_inputs, generate_email_verifier_
                                generate_email_verifier_inputs_from_dkim_result)
 from .app import decode_app_outputs, expected_app_output, generate_app_inputs  # noqa: F401
 from . import hash  # noqa: F401,E402
+from .registry import KeyRegistry  # noqa: F401,E402
 from .engine import AssertFailed, Context, Verifier, Zkey, device_count, proof_to_json, verify, verify_batch  # noqa: F401
 from .engine import ptau_info, ptau_toy, verify_zkey  # noqa: F401
 from .engine import ptau_contribute, ptau_new, ptau_prepare, ptau_report, verify_ptau  # noqa: F401

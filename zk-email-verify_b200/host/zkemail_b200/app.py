@@ -26,7 +26,11 @@ A public part may instead publish a hash of what it matched, with `"reveal"`:
         one output: Poseidon(2)([that hash, salt]), the salt a private external input {"name": "senderSalt", "isPublic": false}
 
 `"reveal": "bytes"` is the default.  External inputs are public unless `"isPublic": false`; private ones come after the
-start indices in the witness.  expected_app_output gives the value a verifier compares an output with."""
+start indices in the witness.  expected_app_output gives the value a verifier compares an output with.
+
+`"keyRegistryDepth": d` (1..32) hides the signing key too: the first output is then `registryRoot`, the root of a
+KeyRegistry (registry.py) that holds the key's pubkeyHash, instead of pubkeyHash itself.  generate_app_inputs takes the
+registry as params={"registry": reg} and fills the private inputs registryIndex and registrySiblings."""
 from __future__ import annotations
 import re
 
@@ -104,6 +108,12 @@ def generate_app_inputs(raw_email_or_dkim_result, spec: dict, external_inputs: d
     DKIM key `resolver`.  Raises ValueError naming the regex that does not match."""
     params = dict(params or {})
     resolver = params.pop("resolver", None)
+    registry = params.pop("registry", None)
+    depth = int(spec.get("keyRegistryDepth", 0))
+    if depth and registry is None:
+        raise ValueError(f'the spec has "keyRegistryDepth": {depth}: pass params={{"registry": KeyRegistry}}')
+    if depth and registry.depth != depth:
+        raise ValueError(f"the registry has depth {registry.depth}, the spec keyRegistryDepth {depth}")
     if isinstance(raw_email_or_dkim_result, DKIMVerificationResult):
         dk = raw_email_or_dkim_result
     else:
@@ -135,13 +145,20 @@ def generate_app_inputs(raw_email_or_dkim_result, spec: dict, external_inputs: d
             inputs[name] = pack_bytes(data, int(ei["maxLength"]))
         else:
             inputs[name] = str(int(v, 0) if isinstance(v, str) else int(v))
+    if depth:
+        from .hash import poseidon_large
+        n, k = int(spec.get("n", 121)), int(spec.get("k", 17))
+        index, siblings = registry.path(registry.index_of(poseidon_large(dk.publicKey, (k + 1) // 2, 2 * n)))
+        inputs["registryIndex"] = str(index)
+        inputs["registrySiblings"] = [str(x) for x in siblings]
     return inputs
 
 
 def decode_app_outputs(spec: dict, public_signals) -> dict:
     """Public signals of an app proof (snarkjs public.json order) -> {name: value}: revealed substrings and packed
     external inputs as strings, every other signal as an int (hashed and committed parts included; the masks as lists of
-    byte values).  Private external inputs are not public signals."""
+    byte values).  Private external inputs are not public signals.  With keyRegistryDepth the first signal is
+    registryRoot instead of pubkeyHash."""
     sig = [int(x) for x in public_signals]
     pos = 0
 
@@ -154,7 +171,7 @@ def decode_app_outputs(spec: dict, public_signals) -> dict:
 
     H = int(spec.get("maxHeadersLength", MAX_HEADER_PADDED_BYTES))
     Bd = int(spec.get("maxBodyLength", MAX_BODY_PADDED_BYTES))
-    out = {"pubkeyHash": take(1)[0]}
+    out = {"registryRoot" if spec.get("keyRegistryDepth") else "pubkeyHash": take(1)[0]}
     if spec.get("exposeHeaderHash", True):
         out["shaHi"], out["shaLo"] = take(2)
     if spec.get("enableHeaderMasking"):

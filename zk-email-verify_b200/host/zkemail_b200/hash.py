@@ -5,6 +5,7 @@
     poseidon_large(value, num_chunks, bits_per_chunk) poseidonLarge: the little-endian chunks of value, hashed once
     poseidon_modular(inputs)                          poseidonModular: chunks of 16 hashed, the chunk hashes folded left
                                                       to right with Poseidon(2) - the PoseidonModular template
+    poseidon_batch(rows, device=0)                    Poseidon of every row (1..16 elements, one width) on the GPU
 
 Inputs are reduced modulo r as circomlibjs does; outputs are ints below r."""
 from __future__ import annotations
@@ -45,4 +46,22 @@ def poseidon_modular(inputs) -> int:
     return out
 
 
-__all__ = ["poseidon", "poseidon_large", "poseidon_modular"]
+def poseidon_batch(rows, device: int = 0) -> list[int]:
+    """[poseidon(row) for row in rows] on the GPU (zke_poseidon_batch): every row has the same width 1..16; values are
+    reduced modulo r like poseidon's."""
+    rows = [[int(x) % FR_MODULUS for x in r] for r in rows]
+    if not rows:
+        return []
+    width = len(rows[0])
+    if not 1 <= width <= CHUNK_SIZE or any(len(r) != width for r in rows):
+        raise ValueError(f"every row needs the same width of 1 to {CHUNK_SIZE} inputs")
+    data = b"".join(v.to_bytes(32, "little") for r in rows for v in r)
+    out = ctypes.create_string_buffer(32 * len(rows))
+    err = ctypes.create_string_buffer(L.ERRCAP)
+    if L.zke_poseidon_batch(data, width, len(rows), device, out, err, L.ERRCAP) != 0:
+        raise L.ZkeError(err.value.decode())
+    raw = out.raw
+    return [int.from_bytes(raw[32 * i:32 * i + 32], "little") for i in range(len(rows))]
+
+
+__all__ = ["poseidon", "poseidon_large", "poseidon_modular", "poseidon_batch"]

@@ -1,0 +1,146 @@
+"""Merkle registry of DKIM keys: the tree an app with `"keyRegistryDepth": d` proves its signing key is a leaf of.
+
+A leaf is a key's pubkeyHash - poseidon_large(modulus, ceil(k / 2), 2n), what EmailVerifier outputs - and a node is
+H(l, r) = Poseidon(2)([l, r]).  With m leaves and depth d, positions m .. 2^d - 1 hold 0: level l stores ceil(m / 2^l)
+nodes, a missing right child at level l is zeros[l] (zeros[0] = 0, zeros[l + 1] = H(zeros[l], zeros[l])), and the root is
+level d's single node.  Bit l of a leaf's index is 1 when its ancestor at level l is a right child.  The leaves and the
+tree are computed on the GPU (zke_pubkey_hashes, zke_merkle_build).
+
+The root says "signed by some key in this set" and nothing about which key, so nothing about which domain: a verifier
+compares a proof's registryRoot with the root of the registry it trusts."""
+from __future__ import annotations
+import base64
+import ctypes
+import json
+import re
+
+from . import _lib as L
+from .circuit import FR_MODULUS
+from .dkim import parse_tag_list
+
+
+def _modulus(key) -> int:
+    """An RSA modulus from an int or a DKIM TXT record (its `p=` tag, read as dkim.py reads DNS records)."""
+    if isinstance(key, int):
+        return key
+    from cryptography.hazmat.primitives import serialization
+    from cryptography.hazmat.primitives.asymmetric import rsa
+    tags = parse_tag_list(key.decode() if isinstance(key, bytes) else str(key))
+    if not tags.get("p"):
+        raise ValueError("DKIM record has no p= tag")
+    pub = serialization.load_der_public_key(base64.b64decode(re.sub(r"\s+", "", tags["p"])))
+    if not isinstance(pub, rsa.RSAPublicKey):
+        raise ValueError("DKIM record does not hold an RSA key")
+    return pub.public_numbers().n
+
+
+def _ints(raw: bytes, count: int) -> list[int]:
+    return [int.from_bytes(raw[32 * i:32 * i + 32], "little") for i in range(count)]
+
+
+def pubkey_hashes(keys, n: int = 121, k: int = 17, device: int = 0) -> list[int]:
+    """The pubkeyHash of each key (moduli or DKIM TXT records) on the GPU."""
+    moduli = [_modulus(x) for x in keys]
+    if not moduli:
+        return []
+    mbytes = max(1, (n * k + 7) // 8, max((m.bit_length() + 7) // 8 for m in moduli))
+    data = b"".join(m.to_bytes(mbytes, "little") for m in moduli)
+    out = ctypes.create_string_buffer(32 * len(moduli))
+    err = ctypes.create_string_buffer(L.ERRCAP)
+    if L.zke_pubkey_hashes(data, len(moduli), mbytes, n, k, device, out, err, L.ERRCAP) != 0:
+        raise L.ZkeError(err.value.decode())
+    return _ints(out.raw, len(moduli))
+
+
+def merkle_levels(leaves, depth: int, device: int = 0) -> list[list[int]]:
+    """Every level of the tree over `leaves` (level 0 = the leaves, the last level = [root]), built on the GPU."""
+    leaves = [int(x) for x in leaves]
+    data = b"".join(x.to_bytes(32, "little") if 0 <= x < FR_MODULUS else b"\xff" * 32 for x in leaves)
+    err = ctypes.create_string_buffer(L.ERRCAP)
+    need = L.zke_merkle_build(data, len(leaves), depth, device, None, 0, err, L.ERRCAP)
+    if need < 0:
+        raise L.ZkeError(err.value.decode())
+    buf = ctypes.create_string_buffer(need)
+    if L.zke_merkle_build(data, len(leaves), depth, device, buf, need, err, L.ERRCAP) != need:
+        raise L.ZkeError(err.value.decode())
+    flat, levels, pos, m = _ints(buf.raw, need // 32), [], 0, len(leaves)
+    for lvl in range(depth + 1):
+        size = -(-m // (1 << lvl))
+        levels.append(flat[pos:pos + size])
+        pos += size
+    return levels
+
+
+class KeyRegistry:
+    """A registry of DKIM keys: depth d, the levels of its tree.  build() and from_leaves() compute them on the GPU; the
+    constructor only checks shapes."""
+
+    def __init__(self, depth: int, levels):
+        if not isinstance(depth, int) or not 1 <= depth <= 32:
+            raise ValueError(f"depth must be 1..32, not {depth!r}")
+        levels = [[int(x) for x in lvl] for lvl in levels]
+        if len(levels) != depth + 1 or not levels[0] or len(levels[0]) > 1 << depth:
+            raise ValueError(f"a tree of depth {depth} has {depth + 1} levels and 1 to 2^{depth} leaves")
+        m = len(levels[0])
+        for lvl, nodes in enumerate(levels):
+            if len(nodes) != -(-m // (1 << lvl)):
+                raise ValueError(f"level {lvl} holds {len(nodes)} nodes, not ceil({m} / 2^{lvl})")
+        self.depth, self.levels = depth, levels
+        self._zeros = None
+
+    @classmethod
+    def build(cls, keys, depth: int, n: int = 121, k: int = 17, device: int = 0) -> "KeyRegistry":
+        """The registry of `keys` (RSA moduli or DKIM TXT records `v=DKIM1; k=rsa; p=...`), in that order."""
+        return cls.from_leaves(pubkey_hashes(keys, n, k, device), depth, device)
+
+    @classmethod
+    def from_leaves(cls, leaves, depth: int, device: int = 0) -> "KeyRegistry":
+        return cls(depth, merkle_levels(leaves, depth, device))
+
+    @property
+    def root(self) -> int:
+        return self.levels[-1][0]
+
+    @property
+    def leaves(self) -> list[int]:
+        return self.levels[0]
+
+    def index_of(self, pubkey_hash: int) -> int:
+        """Index of the first leaf equal to pubkey_hash; ValueError if the key is not in the registry."""
+        try:
+            return self.levels[0].index(int(pubkey_hash))
+        except ValueError:
+            raise ValueError("the key (its pubkeyHash) is not in the registry") from None
+
+    def zeros(self) -> list[int]:
+        if self._zeros is None:
+            from .hash import poseidon
+            z = [0]
+            for _ in range(self.depth):
+                z.append(poseidon([z[-1], z[-1]]))
+            self._zeros = z
+        return self._zeros
+
+    def path(self, i: int) -> tuple[int, list[int]]:
+        """(i, siblings): the authentication path of leaf i, from the leaf's sibling up (the circuit's registryIndex and
+        registrySiblings)."""
+        if not 0 <= i < len(self.levels[0]):
+            raise IndexError(f"leaf {i} is not in a registry of {len(self.levels[0])} keys")
+        sib, j = [], i
+        for lvl in range(self.depth):
+            s = j ^ 1
+            sib.append(self.levels[lvl][s] if s < len(self.levels[lvl]) else self.zeros()[lvl])
+            j >>= 1
+        return i, sib
+
+    def to_json(self) -> str:
+        """The depth and the leaves; from_json rebuilds the tree on the GPU."""
+        return json.dumps({"depth": self.depth, "leaves": [str(x) for x in self.levels[0]]})
+
+    @classmethod
+    def from_json(cls, text: str, device: int = 0) -> "KeyRegistry":
+        d = json.loads(text)
+        return cls.from_leaves([int(x) for x in d["leaves"]], int(d["depth"]), device)
+
+
+__all__ = ["KeyRegistry", "pubkey_hashes", "merkle_levels"]

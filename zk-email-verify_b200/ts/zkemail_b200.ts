@@ -23,6 +23,9 @@ const zke_aggregate = lib.func('int64_t zke_aggregate(void*, const char*, size_t
 const zke_agg_verify = lib.func('int zke_agg_verify(const char*, const char*, size_t, const uint8_t*, const uint8_t*, size_t, char*, size_t)');
 
 const zke_poseidon_hash = lib.func('int zke_poseidon_hash(const uint8_t*, size_t, uint8_t*)');
+const zke_poseidon_batch = lib.func('int zke_poseidon_batch(const uint8_t*, uint32_t, size_t, int, uint8_t*, char*, size_t)');
+const zke_pubkey_hashes = lib.func('int zke_pubkey_hashes(const uint8_t*, size_t, uint32_t, uint32_t, uint32_t, int, uint8_t*, char*, size_t)');
+const zke_merkle_build = lib.func('int64_t zke_merkle_build(const uint8_t*, size_t, uint32_t, int, uint8_t*, size_t, char*, size_t)');
 
 const cstr = (b: Buffer) => b.toString('utf8', 0, b.indexOf(0));
 type Entry = { circuit: unknown; zkey: unknown; ctx: unknown };
@@ -159,4 +162,46 @@ export function poseidonModular(inputs: bigint[]): bigint {
   }
   if (out === null) throw new Error('No inputs provided');
   return out;
+}
+
+/** The key registry on the GPU (zke_poseidon_batch, zke_pubkey_hashes, zke_merkle_build): field elements as bigints. */
+const fromLe32 = (b: Buffer, i: number) => {
+  let x = 0n;
+  for (let j = 31; j >= 0; --j) x = (x << 8n) | BigInt(b[32 * i + j]);
+  return x;
+};
+const toLe = (x: bigint, n: number) => {
+  const b = Buffer.alloc(n);
+  for (let j = 0; j < n; ++j) { b[j] = Number(x & 0xffn); x >>= 8n; }
+  return b;
+};
+export function poseidonBatch(rows: bigint[][], device = 0): bigint[] {
+  if (rows.length === 0) return [];
+  const out = Buffer.alloc(32 * rows.length), err = Buffer.alloc(4096);
+  const data = Buffer.concat(rows.flat().map((x) => toLe(((x % R) + R) % R, 32)));
+  if (zke_poseidon_batch(data, rows[0].length, rows.length, device, out, err, err.length) !== 0) throw new Error(cstr(err));
+  return rows.map((_, i) => fromLe32(out, i));
+}
+export function pubkeyHashes(moduli: bigint[], n = 121, k = 17, device = 0): bigint[] {
+  if (moduli.length === 0) return [];
+  const bytes = Math.ceil((n * k) / 8);
+  const out = Buffer.alloc(32 * moduli.length), err = Buffer.alloc(4096);
+  if (zke_pubkey_hashes(Buffer.concat(moduli.map((m) => toLe(m, bytes))), moduli.length, bytes, n, k, device, out, err, err.length) !== 0)
+    throw new Error(cstr(err));
+  return moduli.map((_, i) => fromLe32(out, i));
+}
+/** Every level of the registry tree, leaves first, root last. */
+export function merkleBuild(leaves: bigint[], depth: number, device = 0): bigint[][] {
+  const err = Buffer.alloc(4096), data = Buffer.concat(leaves.map((x) => toLe(x, 32)));
+  const need = Number(zke_merkle_build(data, leaves.length, depth, device, null, 0, err, err.length));
+  if (need < 0) throw new Error(cstr(err));
+  const buf = Buffer.alloc(need);
+  if (Number(zke_merkle_build(data, leaves.length, depth, device, buf, need, err, err.length)) !== need) throw new Error(cstr(err));
+  const levels: bigint[][] = [];
+  for (let l = 0, pos = 0; l <= depth; ++l) {
+    const size = Math.ceil(leaves.length / 2 ** l);
+    levels.push(Array.from({ length: size }, (_, i) => fromLe32(buf, pos + i)));
+    pos += size;
+  }
+  return levels;
 }
