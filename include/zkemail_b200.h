@@ -61,7 +61,9 @@ zke_circuit* zke_circuit_build_regex(const char* const* parts, const uint8_t* is
  * absent: no registry) hides the signing key: pubkeyHash stays private and is proven a leaf of a Poseidon(2) Merkle tree
  * of depth d (zke_merkle_build), whose root `registryRoot` is published in pubkeyHash's place; the private inputs
  * registryIndex and registrySiblings[d] come last.  It is refused with publicPubkey, and the three names are then
- * reserved.  Signal order: outputs (pubkeyHash or registryRoot, shaHi, shaLo, masks, regex outputs, emailNullifier),
+ * reserved.  `keyDomain` (with keyRegistryDepth) names the output of a public header regex part of maxLength <= 255
+ * whose matched bytes D bind the leaf to a domain: the leaf is Poseidon(2)([Poseidon(9)(D's packed words, zero-padded to
+ * 9), pubkeyHash]) (zke_domain_key_leaves) instead of pubkeyHash; it adds no signal.  Signal order: outputs (pubkeyHash or registryRoot, shaHi, shaLo, masks, regex outputs, emailNullifier),
  * public inputs (external inputs, pubkey if public), the EmailVerifier inputs, the index inputs, private external inputs,
  * then registryIndex and registrySiblings.  A malformed spec is refused with a message naming the field. */
 zke_circuit* zke_circuit_build_app(const char* spec_json, char* err, size_t errcap);
@@ -170,6 +172,11 @@ int zke_poseidon_hash(const uint8_t* inputs, size_t n, uint8_t* out);
  * zke_pubkey_hashes: the pubkeyHash of each of `count` RSA moduli (modulus_bytes each, little-endian): k limbs of n
  *   bits, merged in pairs as PoseidonLarge does, through Poseidon(ceil(k / 2)).  Refuses k outside 17..32, 2n >= 251
  *   and a modulus >= 2^(n k).  Returns 0.
+ * zke_domain_key_leaves: the domain-bound leaf of each of `count` (domain, modulus) pairs, Poseidon(2)([domainHash,
+ *   pubkeyHash]) with domainHash = Poseidon(9) of the domain's 9 packed words (PackBytes(D, 255)).  `domains` holds
+ *   count rows of 255 bytes: the name, lower-case ASCII without a trailing dot, then zero padding.  Refuses what
+ *   zke_pubkey_hashes refuses, and an empty row, a zero byte inside the name, a byte >= 0x80 or in A-Z, and a trailing
+ *   dot, naming the first such row.  Returns 0.
  * zke_merkle_build: every level of the tree of depth 1..32 over count <= 2^depth leaves (below r), node hash
  *   H(l, r) = Poseidon(2)([l, r]).  Level l holds ceil(count / 2^l) nodes, a missing right child at level l is
  *   zeros[l] (zeros[0] = 0, zeros[l + 1] = H(zeros[l], zeros[l])); levels are written one after the other from the
@@ -178,6 +185,8 @@ int zke_poseidon_hash(const uint8_t* inputs, size_t n, uint8_t* out);
 int zke_poseidon_batch(const uint8_t* inputs, uint32_t width, size_t count, int device, uint8_t* out, char* err, size_t errcap);
 int zke_pubkey_hashes(const uint8_t* moduli, size_t count, uint32_t modulus_bytes, uint32_t n, uint32_t k, int device,
                       uint8_t* out, char* err, size_t errcap);
+int zke_domain_key_leaves(const uint8_t* moduli, size_t count, uint32_t modulus_bytes, uint32_t n, uint32_t k,
+                          const uint8_t* domains, int device, uint8_t* out, char* err, size_t errcap);
 int64_t zke_merkle_build(const uint8_t* leaves, size_t count, uint32_t depth, int device, uint8_t* levels, size_t cap,
                          char* err, size_t errcap);
 double zke_registry_device_ms(void);

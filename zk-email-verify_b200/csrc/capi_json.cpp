@@ -215,7 +215,8 @@ const uint32_t MAX_EXTERNAL_BYTES = 1u << 16;
 gadgets::AppSpec app_spec_of(const JV& s) {
     only_keys(s, "spec", {"maxHeadersLength", "maxBodyLength", "n", "k", "ignoreBodyHashCheck", "enableHeaderMasking",
                           "enableBodyMasking", "removeSoftLineBreaks", "publicPubkey", "regexStyle", "exposeHeaderHash",
-                          "regexes", "externalInputs", "emailNullifier", "shaPrecomputeSelector", "keyRegistryDepth"});
+                          "regexes", "externalInputs", "emailNullifier", "shaPrecomputeSelector", "keyRegistryDepth",
+                          "keyDomain"});
     gadgets::AppSpec a;
     gadgets::EmailVerifierParams& ev = a.ev;
     if (const JV* v = s.get("maxHeadersLength")) ev.max_headers_length = uint_of(*v, "maxHeadersLength");
@@ -241,6 +242,10 @@ gadgets::AppSpec app_spec_of(const JV& s) {
     if (const JV* v = s.get("keyRegistryDepth")) {
         a.key_registry_depth = uint_of(*v, "keyRegistryDepth");
         if (a.key_registry_depth > 32) throw std::runtime_error("keyRegistryDepth: at most 32, not " + v->s);
+    }
+    if (s.get("keyDomain")) {
+        a.key_domain = str_of(s, "keyDomain", "");
+        if (a.key_domain.empty()) throw std::runtime_error("keyDomain: empty name");
     }
     if (const JV* rs = array_of(s, "regexes")) {
         for (size_t r = 0; r < rs->arr.size(); ++r) {

@@ -859,6 +859,19 @@ LC binary_merkle_root(Builder& b, const LC& leaf, const LC& index, const LCVec& 
     return cur;
 }
 
+LC domain_key_leaf(Builder& b, const LCVec& words, const LC& key_hash) {
+    ScopeGuard g(b, "DomainKeyLeaf");
+    if (words.empty() || words.size() > 9) throw std::runtime_error("DomainKeyLeaf: 1..9 packed words");
+    const bool record = b.materialize_linear;           // a record needs its inputs as signals
+    // a record takes variables only: one signal constrained to zero fills every padding word (a record may repeat an
+    // input), so the hash is PoseidonModular(PackBytes(D, 255)) whatever the part's maxLength
+    LCVec in(9);
+    const Var zero = words.size() < 9 ? as_var(b, LC()) : 0;
+    for (size_t i = 0; i < 9; ++i) in[i] = i < words.size() ? LC(as_var(b, words[i])) : LC(zero);
+    LC domain_hash = poseidon(b, in, record);
+    return poseidon(b, {LC(as_var(b, domain_hash)), LC(as_var(b, key_hash))}, record);
+}
+
 // ---------------------------------------------------------------- helpers/remove-soft-line-breaks.circom
 LC remove_soft_line_breaks(Builder& b, const LCVec& encoded, const LCVec& decoded) {
     ScopeGuard g(b, "RemoveSoftLineBreaks");
@@ -1012,6 +1025,23 @@ Circuit build_email_app(const AppSpec& A, bool materialize_linear) {
         for (auto& rv : reveals[r]) { check_registry("regexes[" + std::to_string(r) + "].name", rv.out); check_registry("regexes[" + std::to_string(r) + "].name", rv.index); }
     for (size_t e = 0; e < A.external_inputs.size(); ++e) check_registry("externalInputs[" + std::to_string(e) + "].name", A.external_inputs[e].name);
 
+    // keyDomain: the public header part whose bytes the registry leaf binds to the key
+    size_t kd_regex = 0, kd_part = 0;
+    const bool domain_bound = !A.key_domain.empty();
+    if (domain_bound) {
+        const std::string& kd = A.key_domain;
+        if (!depth) throw std::runtime_error("keyDomain: binds the registry leaf to a domain, so it needs keyRegistryDepth");
+        bool found = false;
+        for (size_t r = 0; r < A.regexes.size() && !found; ++r)
+            for (size_t q = 0; q < reveals[r].size() && !found; ++q)
+                if (reveals[r][q].out == kd) { found = true; kd_regex = r; kd_part = q; }
+        if (!found) throw std::runtime_error("keyDomain: '" + kd + "' is not the output name of a public regex part");
+        if (A.regexes[kd_regex].body)
+            throw std::runtime_error("keyDomain: '" + kd + "' is a body regex part; the domain must come from the signed header");
+        const uint32_t ml = reveals[kd_regex][kd_part].max_length;
+        if (ml > 255) throw std::runtime_error("keyDomain: '" + kd + "' has maxLength " + std::to_string(ml) + "; a domain has at most 255 bytes");
+    }
+
     Builder b("EmailVerifier");
     b.materialize_linear = materialize_linear;
     if (P.regex_style >= 0) b.regex_style = P.regex_style;
@@ -1116,11 +1146,14 @@ Circuit build_email_app(const AppSpec& A, bool materialize_linear) {
         }
     }
     LC key_hash = poseidon_large(b, n, pubkey);                          // :173
-    if (depth) key_hash = binary_merkle_root(b, key_hash, registry_index, registry_siblings);
-    b.assign_output(pubkey_hash, key_hash);
+    if (!domain_bound) {                 // a domain-bound leaf needs the domain's words: its root follows the regexes
+        if (depth) key_hash = binary_merkle_root(b, key_hash, registry_index, registry_siblings);
+        b.assign_output(pubkey_hash, key_hash);
+    }
     if (A.regexes.empty() && !A.email_nullifier) return b.finalize();
 
     ScopeGuard ag(b, A.scope);
+    LCVec domain_words;                                                  // keyDomain's packed words
     for (size_t r = 0; r < A.regexes.size(); ++r) {                      // the app's regexes (UsageGuide step 2)
         const AppRegex& ar = A.regexes[r];
         const LCVec& msg = ar.body ? (P.remove_soft_line_breaks ? decoded_in : email_body) : email_header;
@@ -1137,17 +1170,26 @@ Circuit build_email_app(const AppSpec& A, bool materialize_linear) {
             LCVec reveal(rx.begin() + 1 + q * msg.size(), rx.begin() + 1 + (q + 1) * msg.size());
             const Reveal& rv = reveals[r][q];
             LCVec packs = pack_regex_reveal(b, reveal, reveal_index[r][q], rv.max_length);
+            const bool is_domain = domain_bound && r == kd_regex && q == kd_part;
             if (rv.reveal == REVEAL_BYTES) {
                 for (size_t i = 0; i < packs.size(); ++i) b.assign_output(reveal_out[r][q][i], packs[i]);
+                if (is_domain) domain_words = to_lcs(reveal_out[r][q]);
                 continue;
             }
             // hash / commit: the packed words stay intermediate signals; the Poseidon instances are recorded for the
             // engine's native permutation (circuit.hpp: PoseidonBlock)
             for (LC& p : packs) p = b.signal(p);
+            if (is_domain) domain_words = packs;
             LC h = poseidon_modular(b, packs, true);
             if (rv.reveal == REVEAL_COMMIT) h = poseidon(b, {h, LC(external_first[rv.salt])}, true);
             b.assign_output(reveal_out[r][q][0], h);
         }
+    }
+    if (domain_bound) {
+        // select_regex_reveal pins the exact matched run (a non-zero first byte after a zero, zeros past it), so the
+        // words are the whole part D; the leaf ties D to the key that verified the signature
+        LC leaf = domain_key_leaf(b, domain_words, key_hash);
+        b.assign_output(pubkey_hash, binary_merkle_root(b, leaf, registry_index, registry_siblings));
     }
     if (A.email_nullifier) b.assign_output(nullifier, email_nullifier(b, n, signature));   // helpers/email-nullifier.circom
     return b.finalize();

@@ -64,6 +64,9 @@ LC remove_soft_line_breaks(Builder& b, const LCVec& encoded, const LCVec& decode
 // root of a binary Poseidon(2) Merkle tree of depth siblings.size() (1..32) from a leaf, its index (bit l set: the node at
 // level l is a right child; index < 2^depth is enforced) and the authentication path; each node hash is recorded
 LC binary_merkle_root(Builder& b, const LC& leaf, const LC& index, const LCVec& siblings);
+// a registry leaf bound to a domain: Poseidon(2)([Poseidon(9)(words zero-padded to 9), key_hash]), words = the packed
+// domain (at most 9, PackBytes of at most 255 bytes); both hashes are recorded
+LC domain_key_leaf(Builder& b, const LCVec& words, const LC& key_hash);
 
 // ---- lib/ ------------------------------------------------------------------------------------
 LCVec sha256_general(Builder& b, const LCVec& padded_in_bits, const LC& padded_in_length_bits,
@@ -144,6 +147,9 @@ struct AppSpec {
     // 1..32: pubkeyHash stays private and is proven a leaf of a Merkle registry of keys; the output registryRoot takes
     // its place, the private inputs registryIndex and registrySiblings[depth] come last.  0: no registry
     uint32_t key_registry_depth = 0;
+    // with a registry: the output name of a public header regex part (maxLength <= 255) whose matched bytes D bind the
+    // leaf to a domain, leaf = domain_key_leaf(D's packed words, pubkeyHash).  Empty: the leaf is pubkeyHash
+    std::string key_domain;
 };
 Circuit build_email_app(const AppSpec& spec, bool materialize_linear = true);
 

@@ -1,5 +1,5 @@
 // Batched Poseidon and the Merkle registry of DKIM keys (include/zkemail_b200.h: zke_poseidon_batch, zke_pubkey_hashes,
-// zke_merkle_build).
+// zke_domain_key_leaves, zke_merkle_build).
 //
 // One thread runs one Poseidon instance: the Merkle node hash (width 3) with its state in registers, the other widths
 // from one instantiation that takes the width at run time (its state in the thread's stack frame).  The round constants and the MDS matrix of the width come from
@@ -126,34 +126,39 @@ __device__ __forceinline__ void bit_field(const uint8_t* m, uint32_t len, uint32
     }
 }
 
-// PoseidonLarge leaves: modulus i (mlen bytes, little-endian) -> its k limbs of n bits, merged in pairs (limb 2j + limb
-// 2j+1 * 2^n, the last limb alone for odd k) = the 2n-bit chunks of the modulus, hashed with Poseidon(T - 1), T - 1 =
-// ceil(k / 2).  A modulus with a bit at or above n k goes to *bad.
-__global__ void __launch_bounds__(REG_THREADS)
-pubkey_hash_kernel(const uint8_t* __restrict__ moduli, uint64_t count, uint32_t mlen, uint32_t n, uint32_t k,
-                   const uint8_t* __restrict__ consts, int r_p, uint8_t* __restrict__ out, uint32_t* __restrict__ bad) {
-    extern __shared__ uint4 smem[];
-    Fr* sh = reinterpret_cast<Fr*>(smem);
+// the PoseidonLarge input of one modulus (mlen bytes, little-endian) into st[1..t-1], t - 1 = ceil(k / 2): its k limbs
+// of n bits, merged in pairs (limb 2j + limb 2j+1 * 2^n, the last limb alone for odd k) = the 2n-bit chunks of the
+// modulus.  A modulus with a bit at or above n k sets *bad.
+__device__ __forceinline__ void pubkey_chunks(const uint8_t* m, uint32_t mlen, uint32_t n, uint32_t k, Fr* st, bool* bad) {
     const int t = (int)(k + 1) / 2 + 1;
-    stage_constants(sh, consts, n_constants(t, r_p));
-    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= count) return;
-    const uint8_t* m = moduli + (uint64_t)mlen * i;
     const uint32_t nk = n * k;
-    bool b = false;
     for (uint32_t byte = nk >> 3; byte < mlen; ++byte) {
         const uint32_t first = byte == (nk >> 3) ? (nk & 7) : 0;
-        if (m[byte] >> first) b = true;
+        if (m[byte] >> first) *bad = true;
     }
-    Fr st[MAX_T];
-    st[0] = Fr::zero();
 #pragma unroll 1
     for (int j = 1; j < t; ++j) {
         const uint32_t off = 2 * n * (j - 1);
         uint32_t w[8];
         bit_field(m, mlen, off, min(2 * n, nk - off), w);
-        st[j] = fr_in(w, &b);
+        st[j] = fr_in(w, bad);
     }
+}
+
+// PoseidonLarge leaves: out[i] = pubkeyHash of modulus i; the first modulus with a bit at or above n k goes to *bad
+__global__ void __launch_bounds__(REG_THREADS)
+pubkey_hash_kernel(const uint8_t* __restrict__ moduli, uint64_t count, uint32_t mlen, uint32_t n, uint32_t k,
+                   const uint8_t* __restrict__ consts, int r_p, uint8_t* __restrict__ out, uint32_t* __restrict__ bad) {
+    extern __shared__ uint4 smem[];
+    Fr* sh = reinterpret_cast<Fr*>(smem);
+    stage_constants(sh, consts, n_constants((int)(k + 1) / 2 + 1, r_p));
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= count) return;
+    const int t = (int)(k + 1) / 2 + 1;
+    bool b = false;
+    Fr st[MAX_T];
+    st[0] = Fr::zero();
+    pubkey_chunks(moduli + (uint64_t)mlen * i, mlen, n, k, st, &b);
     if (b) atomicMin(bad, (uint32_t)min(i, (uint64_t)NO_BAD - 1));
     fr_store(out + 32ull * i, permute<0>(st, t, sh, sh + (8 + r_p) * t, r_p));
 }
@@ -161,6 +166,75 @@ pubkey_hash_kernel(const uint8_t* __restrict__ moduli, uint64_t count, uint32_t 
 __device__ __forceinline__ Fr node_hash(const Fr& l, const Fr& r, const Fr* rc, const Fr* mds, int r_p) {
     Fr st[3] = {Fr::zero(), l, r};
     return permute<3>(st, 3, rc, mds, r_p);
+}
+
+// A domain row: DOMAIN_BYTES bytes, the name then zero padding (the byte image of PackBytes(D, 255)), packed into
+// DOMAIN_WORDS words of 31 bytes, little-endian.  Canonical: 1..255 bytes, ASCII without upper-case letters, no zero
+// byte inside the name, no trailing dot.
+static const uint32_t DOMAIN_BYTES = 255, DOMAIN_WORDS = 9, DOMAIN_T = DOMAIN_WORDS + 1;
+
+__device__ __forceinline__ bool domain_canonical(const uint8_t* d) {
+    bool ok = d[0] != 0, ended = false;
+    uint8_t last = 0;
+#pragma unroll 1
+    for (uint32_t j = 0; j < DOMAIN_BYTES; ++j) {
+        const uint8_t c = d[j];
+        if (c == 0) { ended = true; continue; }
+        if (ended || c >= 0x80 || (c >= 'A' && c <= 'Z')) ok = false;
+        last = c;
+    }
+    return ok && last != '.';
+}
+
+// Domain-bound leaves: out[i] = Poseidon(2)([Poseidon(9)(the 9 words of domain row i), pubkeyHash of modulus i]).
+// Shared memory holds the constants of width DOMAIN_T, then those of the key's width tk unless tk == DOMAIN_T (k = 17,
+// 18), then those of width 3.  The first bad modulus goes to *bad_key, the first non-canonical row to *bad_domain.
+__global__ void __launch_bounds__(REG_THREADS)
+domain_key_leaf_kernel(const uint8_t* __restrict__ moduli, const uint8_t* __restrict__ domains, uint64_t count, uint32_t mlen,
+                       uint32_t n, uint32_t k, const uint8_t* __restrict__ consts_d, int r_p_d,
+                       const uint8_t* __restrict__ consts_k, int r_p_k, const uint8_t* __restrict__ consts_2, int r_p_2,
+                       uint8_t* __restrict__ out, uint32_t* __restrict__ bad_key, uint32_t* __restrict__ bad_domain) {
+    extern __shared__ uint4 smem[];
+    const int tk = (int)(k + 1) / 2 + 1;
+    Fr* sh_d = reinterpret_cast<Fr*>(smem);
+    Fr* sh_k = sh_d + n_constants(DOMAIN_T, r_p_d);
+    stage_constants(sh_d, consts_d, n_constants(DOMAIN_T, r_p_d));
+    if (tk == (int)DOMAIN_T) sh_k = sh_d;
+    else stage_constants(sh_k, consts_k, n_constants(tk, r_p_k));
+    Fr* sh_2 = sh_k + n_constants(tk, r_p_k);
+    stage_constants(sh_2, consts_2, n_constants(3, r_p_2));
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= count) return;
+    const uint8_t* d = domains + (uint64_t)DOMAIN_BYTES * i;
+    if (!domain_canonical(d)) atomicMin(bad_domain, (uint32_t)min(i, (uint64_t)NO_BAD - 1));
+    bool b = false;
+    Fr st[MAX_T], domain_hash, key_hash;
+    // one permutation site at a run-time width for the three hashes: a call at a constant width is unrolled with its
+    // state in registers, which takes the kernel from about 50 to about 240 registers
+#pragma unroll 1
+    for (int job = 0; job < 3; ++job) {
+        const Fr* c = job == 0 ? sh_d : job == 1 ? sh_k : sh_2;
+        const int t = job == 0 ? (int)DOMAIN_T : job == 1 ? tk : 3, r_p = job == 0 ? r_p_d : job == 1 ? r_p_k : r_p_2;
+        st[0] = Fr::zero();
+        if (job == 0) {
+#pragma unroll 1
+            for (uint32_t j = 0; j < DOMAIN_WORDS; ++j) {
+                uint32_t w[8];
+                bit_field(d, DOMAIN_BYTES, 248 * j, 248, w);     // below 2^248 < r: never bad
+                st[j + 1] = fr_in(w, &b);
+            }
+        } else if (job == 1) {
+            pubkey_chunks(moduli + (uint64_t)mlen * i, mlen, n, k, st, &b);
+        } else {
+            st[1] = domain_hash;
+            st[2] = key_hash;
+        }
+        const Fr h = permute<0>(st, t, c, c + (8 + r_p) * t, r_p);
+        if (job == 0) domain_hash = h;
+        else if (job == 1) key_hash = h;
+        else fr_store(out + 32ull * i, h);
+    }
+    if (b) atomicMin(bad_key, (uint32_t)min(i, (uint64_t)NO_BAD - 1));
 }
 
 // Levels 1..L of the tree (L <= FUSE_LEVELS): block b owns the nodes under its 2^L leaves.  levels: the whole level
@@ -280,6 +354,28 @@ void set_smem(K kernel, size_t bytes) {
     CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
 }
 
+// the key shapes PoseidonLarge takes (zke_pubkey_hashes, zke_domain_key_leaves)
+void check_key_shape(uint32_t modulus_bytes, uint32_t n, uint32_t k) {
+    if (k < 17 || k > 32) throw std::runtime_error("k must be 17..32 (PoseidonLarge), not " + std::to_string(k));
+    if (n == 0 || 2 * n >= 251) throw std::runtime_error("n must satisfy 0 < 2n < 251 (PoseidonLarge), not " + std::to_string(n));
+    if (modulus_bytes == 0) throw std::runtime_error("modulus_bytes must be positive");
+}
+
+// why a domain row is not canonical (the device only reports which row)
+std::string domain_fault(const uint8_t* d) {
+    if (d[0] == 0) return "is empty";
+    uint32_t len = 0;
+    while (len < dev::DOMAIN_BYTES && d[len]) ++len;
+    for (uint32_t j = len; j < dev::DOMAIN_BYTES; ++j)
+        if (d[j]) return "has a zero byte at " + std::to_string(len) + " inside the name";
+    for (uint32_t j = 0; j < len; ++j) {
+        if (d[j] >= 0x80) return "has a non-ASCII byte at " + std::to_string(j) + " (give the A-label form)";
+        if (d[j] >= 'A' && d[j] <= 'Z') return "has an upper-case byte at " + std::to_string(j);
+    }
+    if (d[len - 1] == '.') return "ends with a dot";
+    return "";
+}
+
 }  // namespace
 
 extern "C" {
@@ -315,9 +411,7 @@ int zke_pubkey_hashes(const uint8_t* moduli, size_t count, uint32_t modulus_byte
                       uint8_t* out, char* err, size_t errcap) {
     try {
         if (!moduli || !out) throw std::runtime_error("null argument");
-        if (k < 17 || k > 32) throw std::runtime_error("k must be 17..32 (PoseidonLarge), not " + std::to_string(k));
-        if (n == 0 || 2 * n >= 251) throw std::runtime_error("n must satisfy 0 < 2n < 251 (PoseidonLarge), not " + std::to_string(n));
-        if (modulus_bytes == 0) throw std::runtime_error("modulus_bytes must be positive");
+        check_key_shape(modulus_bytes, n, k);
         if (count == 0) return 0;
         select_device(device);
         const int t = (int)(k + 1) / 2 + 1;
@@ -337,6 +431,43 @@ int zke_pubkey_hashes(const uint8_t* moduli, size_t count, uint32_t modulus_byte
         const uint32_t b = read_bad(bad);
         if (b != dev::NO_BAD)
             throw std::runtime_error("modulus " + std::to_string(b) + " is not below 2^(n k) = 2^" + std::to_string(n * k));
+        CUDA_OK(cudaMemcpy(out, dout.p, dout.bytes, cudaMemcpyDeviceToHost));
+        return 0;
+    } catch (const std::exception& e) { set_err(err, errcap, e.what()); return -1; }
+}
+
+int zke_domain_key_leaves(const uint8_t* moduli, size_t count, uint32_t modulus_bytes, uint32_t n, uint32_t k,
+                          const uint8_t* domains, int device, uint8_t* out, char* err, size_t errcap) {
+    try {
+        if (!moduli || !domains || !out) throw std::runtime_error("null argument");
+        check_key_shape(modulus_bytes, n, k);
+        if (count == 0) return 0;
+        select_device(device);
+        const int tk = (int)(k + 1) / 2 + 1;
+        WidthConsts Cd(dev::DOMAIN_T), Ck(tk), C2(3);
+        const size_t smem = Cd.smem() + (tk == (int)dev::DOMAIN_T ? 0 : Ck.smem()) + C2.smem();
+        DevBuf dm, dd, dout, bad_key, bad_domain;
+        bad_flag(bad_key);
+        bad_flag(bad_domain);
+        dm.alloc((size_t)modulus_bytes * count);
+        dd.alloc((size_t)dev::DOMAIN_BYTES * count);
+        dout.alloc(32ull * count);
+        CUDA_OK(cudaMemcpy(dm.p, moduli, dm.bytes, cudaMemcpyHostToDevice));
+        CUDA_OK(cudaMemcpy(dd.p, domains, dd.bytes, cudaMemcpyHostToDevice));
+        Timer tm;
+        set_smem(dev::domain_key_leaf_kernel, smem);     // above the 48 KB default once the key has a width of its own (k >= 19)
+        dev::domain_key_leaf_kernel<<<blocks_for(count), dev::REG_THREADS, smem>>>(
+            dm.p, dd.p, count, modulus_bytes, n, k, Cd.buf.p, Cd.r_p, Ck.buf.p, Ck.r_p, C2.buf.p, C2.r_p, dout.p,
+            reinterpret_cast<uint32_t*>(bad_key.p), reinterpret_cast<uint32_t*>(bad_domain.p));
+        ZKE_COUNT_LAUNCH(1);
+        CHECK_LAUNCH();
+        tm.stop();
+        const uint32_t bk = read_bad(bad_key), bd = read_bad(bad_domain);
+        if (bk != dev::NO_BAD)
+            throw std::runtime_error("modulus " + std::to_string(bk) + " is not below 2^(n k) = 2^" + std::to_string(n * k));
+        if (bd != dev::NO_BAD)
+            throw std::runtime_error("domain " + std::to_string(bd) + " is not canonical: it " +
+                                     domain_fault(domains + (size_t)dev::DOMAIN_BYTES * bd));
         CUDA_OK(cudaMemcpy(out, dout.p, dout.bytes, cudaMemcpyDeviceToHost));
         return 0;
     } catch (const std::exception& e) { set_err(err, errcap, e.what()); return -1; }

@@ -60,6 +60,8 @@ LOWER_NATIVE_SHA, LOWER_NATIVE_REGEX, LOWER_COOP_FPMUL, LOWER_NATIVE_POSEIDON = 
 zke_poseidon_hash = _sig("zke_poseidon_hash", c_int, [c_char_p, c_size_t, c_char_p])
 zke_poseidon_batch = _sig("zke_poseidon_batch", c_int, [c_char_p, c_u32, c_size_t, c_int, c_void_p, c_char_p, c_size_t])
 zke_pubkey_hashes = _sig("zke_pubkey_hashes", c_int, [c_char_p, c_size_t, c_u32, c_u32, c_u32, c_int, c_void_p, c_char_p, c_size_t])
+zke_domain_key_leaves = _sig("zke_domain_key_leaves", c_int, [c_char_p, c_size_t, c_u32, c_u32, c_u32, c_char_p, c_int, c_void_p,
+                                                               c_char_p, c_size_t])
 zke_merkle_build = _sig("zke_merkle_build", c_i64, [c_char_p, c_size_t, c_u32, c_int, c_void_p, c_size_t, c_char_p, c_size_t])
 zke_registry_device_ms = _sig("zke_registry_device_ms", ctypes.c_double, [])
 zke_device_count = _sig("zke_device_count", c_int, [])

@@ -30,7 +30,12 @@ start indices in the witness.  expected_app_output gives the value a verifier co
 
 `"keyRegistryDepth": d` (1..32) hides the signing key too: the first output is then `registryRoot`, the root of a
 KeyRegistry (registry.py) that holds the key's pubkeyHash, instead of pubkeyHash itself.  generate_app_inputs takes the
-registry as params={"registry": reg} and fills the private inputs registryIndex and registrySiblings."""
+registry as params={"registry": reg} and fills the private inputs registryIndex and registrySiblings.
+
+`"keyDomain": "<output name of a public header part>"` (with keyRegistryDepth, maxLength <= 255) binds the registry leaf to
+a domain: the leaf is Poseidon(2)([domain_hash(D), pubkeyHash]) for the bytes D that part matched, so the registry must be
+built with KeyRegistry.build_domains from (domain, key) pairs, and registryRoot then proves "signed by a key the registry
+lists for domain D".  D itself is published as the part's reveal mode says (bytes, hash or commit)."""
 from __future__ import annotations
 import re
 
@@ -114,6 +119,12 @@ def generate_app_inputs(raw_email_or_dkim_result, spec: dict, external_inputs: d
         raise ValueError(f'the spec has "keyRegistryDepth": {depth}: pass params={{"registry": KeyRegistry}}')
     if depth and registry.depth != depth:
         raise ValueError(f"the registry has depth {registry.depth}, the spec keyRegistryDepth {depth}")
+    key_domain = spec.get("keyDomain")
+    if depth and bool(key_domain) != registry.domain_bound:
+        raise ValueError(f'the spec has "keyDomain": {key_domain!r}: pass a registry of (domain, key) leaves '
+                         '(KeyRegistry.build_domains)' if key_domain else
+                         'the registry holds (domain, key) leaves: the spec needs "keyDomain"')
+    domain = None
     if isinstance(raw_email_or_dkim_result, DKIMVerificationResult):
         dk = raw_email_or_dkim_result
     else:
@@ -134,6 +145,8 @@ def generate_app_inputs(raw_email_or_dkim_result, spec: dict, external_inputs: d
             raise ValueError(f'regex "{rx["name"]}" does not match the email\'s {rx["location"]}')
         for i, name, _ in public_parts(rx):
             inputs[name + "Index"] = str(m.start(f"p{i}"))
+            if name == key_domain:
+                domain = m.group(f"p{i}")
     external_inputs = external_inputs or {}
     for ei in spec.get("externalInputs", []):
         name = ei["name"]
@@ -146,9 +159,23 @@ def generate_app_inputs(raw_email_or_dkim_result, spec: dict, external_inputs: d
         else:
             inputs[name] = str(int(v, 0) if isinstance(v, str) else int(v))
     if depth:
-        from .hash import poseidon_large
+        from .hash import canonical_domain, domain_words, poseidon, poseidon_large
         n, k = int(spec.get("n", 121)), int(spec.get("k", 17))
-        index, siblings = registry.path(registry.index_of(poseidon_large(dk.publicKey, (k + 1) // 2, 2 * n)))
+        leaf = poseidon_large(dk.publicKey, (k + 1) // 2, 2 * n)
+        if key_domain:
+            # the circuit hashes the matched bytes as they are: a name not in canonical form has no leaf in any registry
+            text = domain.decode("utf-8", errors="replace")
+            try:
+                canonical = canonical_domain(domain) == domain
+            except ValueError:
+                canonical = False
+            if not canonical:
+                raise ValueError(f'{key_domain} "{text}" is not a canonical domain (lower-case ASCII, no trailing dot): '
+                                 "no registry leaf can match it")
+            leaf = poseidon([poseidon(domain_words(domain)), leaf])
+            if leaf not in registry.leaves:
+                raise ValueError(f'the signing key is not registered for domain "{text}"')
+        index, siblings = registry.path(registry.index_of(leaf))
         inputs["registryIndex"] = str(index)
         inputs["registrySiblings"] = [str(x) for x in siblings]
     return inputs

@@ -6,6 +6,8 @@
     poseidon_modular(inputs)                          poseidonModular: chunks of 16 hashed, the chunk hashes folded left
                                                       to right with Poseidon(2) - the PoseidonModular template
     poseidon_batch(rows, device=0)                    Poseidon of every row (1..16 elements, one width) on the GPU
+    domain_hash(domain)                               PoseidonModular(PackBytes(domain, 255)): one Poseidon(9), the
+                                                      domain half of a domain-bound registry leaf
 
 Inputs are reduced modulo r as circomlibjs does; outputs are ints below r."""
 from __future__ import annotations
@@ -64,4 +66,41 @@ def poseidon_batch(rows, device: int = 0) -> list[int]:
     return [int.from_bytes(raw[32 * i:32 * i + 32], "little") for i in range(len(rows))]
 
 
-__all__ = ["poseidon", "poseidon_large", "poseidon_modular", "poseidon_batch"]
+DOMAIN_BYTES = 255           # a DNS name has at most 255 bytes: PackBytes(D, 255) is 9 words
+
+
+def canonical_domain(domain) -> bytes:
+    """The canonical form of a domain name: ASCII (an international name in its A-label form, xn--...), lower case,
+    without a trailing dot, 1..255 bytes and no zero byte.  Lowercases and strips one trailing dot; ValueError otherwise."""
+    if isinstance(domain, str):
+        try:
+            raw = domain.encode("ascii")
+        except UnicodeEncodeError:
+            raise ValueError(f"domain {domain!r} is not ASCII: give an international name in its A-label (xn--) form") from None
+    else:
+        raw = bytes(domain)
+        if any(c >= 0x80 for c in raw):
+            raise ValueError(f"domain {raw!r} is not ASCII: give an international name in its A-label (xn--) form")
+    raw = raw.lower()
+    if raw.endswith(b"."):
+        raw = raw[:-1]
+    if not 1 <= len(raw) <= DOMAIN_BYTES:
+        raise ValueError(f"domain {raw!r} has {len(raw)} bytes; a domain has 1 to {DOMAIN_BYTES}")
+    if 0 in raw:
+        raise ValueError(f"domain {raw!r} holds a zero byte")
+    return raw
+
+
+def domain_words(raw: bytes) -> list[int]:
+    """PackBytes(raw, 255): the 9 little-endian 31-byte words of the zero-padded name (no canonical check)."""
+    raw = raw.ljust(DOMAIN_BYTES, b"\0")
+    return [int.from_bytes(raw[31 * i:31 * i + 31], "little") for i in range(9)]
+
+
+def domain_hash(domain) -> int:
+    """PoseidonModular(PackBytes(canonical_domain(domain), 255)), one Poseidon(9): what a `"reveal": "hash"` part of
+    maxLength 255 publishes for the name, whatever maxLength the part that binds the registry leaf has."""
+    return poseidon(domain_words(canonical_domain(domain)))
+
+
+__all__ = ["poseidon", "poseidon_large", "poseidon_modular", "poseidon_batch", "canonical_domain", "domain_hash"]

@@ -7,7 +7,12 @@ level d's single node.  Bit l of a leaf's index is 1 when its ancestor at level 
 tree are computed on the GPU (zke_pubkey_hashes, zke_merkle_build).
 
 The root says "signed by some key in this set" and nothing about which key, so nothing about which domain: a verifier
-compares a proof's registryRoot with the root of the registry it trusts."""
+compares a proof's registryRoot with the root of the registry it trusts.
+
+A domain-bound registry (build_domains, for specs with `"keyDomain"`) holds (domain, key) pairs instead, as DKIMRegistry's
+isDKIMPublicKeyHashValid(domain, pubkeyHash) does: leaf = Poseidon(2)([domain_hash(domain), pubkeyHash]), with
+domain_hash = PoseidonModular(PackBytes(domain, 255)) (hash.domain_hash).  Its root says "signed by a key the registry
+lists for the domain the proof names".  One key may sit under several domains and one domain may have several keys."""
 from __future__ import annotations
 import base64
 import ctypes
@@ -17,6 +22,7 @@ import re
 from . import _lib as L
 from .circuit import FR_MODULUS
 from .dkim import parse_tag_list
+from .hash import DOMAIN_BYTES, canonical_domain
 
 
 def _modulus(key) -> int:
@@ -43,13 +49,38 @@ def pubkey_hashes(keys, n: int = 121, k: int = 17, device: int = 0) -> list[int]
     moduli = [_modulus(x) for x in keys]
     if not moduli:
         return []
-    mbytes = max(1, (n * k + 7) // 8, max((m.bit_length() + 7) // 8 for m in moduli))
-    data = b"".join(m.to_bytes(mbytes, "little") for m in moduli)
+    data, mbytes = _moduli_image(moduli, n, k)
     out = ctypes.create_string_buffer(32 * len(moduli))
     err = ctypes.create_string_buffer(L.ERRCAP)
     if L.zke_pubkey_hashes(data, len(moduli), mbytes, n, k, device, out, err, L.ERRCAP) != 0:
         raise L.ZkeError(err.value.decode())
     return _ints(out.raw, len(moduli))
+
+
+def _moduli_image(moduli, n: int, k: int) -> tuple[bytes, int]:
+    mbytes = max(1, (n * k + 7) // 8, max((m.bit_length() + 7) // 8 for m in moduli))
+    return b"".join(m.to_bytes(mbytes, "little") for m in moduli), mbytes
+
+
+def domain_key_leaves(pairs, n: int = 121, k: int = 17, device: int = 0) -> list[int]:
+    """The domain-bound leaf of each (domain, key) pair on the GPU (zke_domain_key_leaves); keys are moduli or DKIM TXT
+    records, domains are brought to canonical form (hash.canonical_domain)."""
+    pairs = [(canonical_domain(d), _modulus(x)) for d, x in pairs]
+    if not pairs:
+        return []
+    data, mbytes = _moduli_image([m for _, m in pairs], n, k)
+    rows = b"".join(d.ljust(DOMAIN_BYTES, b"\0") for d, _ in pairs)
+    out = ctypes.create_string_buffer(32 * len(pairs))
+    err = ctypes.create_string_buffer(L.ERRCAP)
+    if L.zke_domain_key_leaves(data, len(pairs), mbytes, n, k, rows, device, out, err, L.ERRCAP) != 0:
+        raise L.ZkeError(err.value.decode())
+    return _ints(out.raw, len(pairs))
+
+
+def domain_key_leaf(domain, key, n: int = 121, k: int = 17) -> int:
+    """One domain-bound leaf on the host: Poseidon(2)([domain_hash(domain), pubkeyHash(key)])."""
+    from .hash import domain_hash, poseidon, poseidon_large
+    return poseidon([domain_hash(domain), poseidon_large(_modulus(key), (k + 1) // 2, 2 * n)])
 
 
 def merkle_levels(leaves, depth: int, device: int = 0) -> list[list[int]]:
@@ -72,10 +103,10 @@ def merkle_levels(leaves, depth: int, device: int = 0) -> list[list[int]]:
 
 
 class KeyRegistry:
-    """A registry of DKIM keys: depth d, the levels of its tree.  build() and from_leaves() compute them on the GPU; the
-    constructor only checks shapes."""
+    """A registry of DKIM keys: depth d, the levels of its tree.  build(), build_domains() and from_leaves() compute them on
+    the GPU; the constructor only checks shapes.  domain_bound: the leaves are (domain, key) leaves (build_domains)."""
 
-    def __init__(self, depth: int, levels):
+    def __init__(self, depth: int, levels, domain_bound: bool = False):
         if not isinstance(depth, int) or not 1 <= depth <= 32:
             raise ValueError(f"depth must be 1..32, not {depth!r}")
         levels = [[int(x) for x in lvl] for lvl in levels]
@@ -86,6 +117,7 @@ class KeyRegistry:
             if len(nodes) != -(-m // (1 << lvl)):
                 raise ValueError(f"level {lvl} holds {len(nodes)} nodes, not ceil({m} / 2^{lvl})")
         self.depth, self.levels = depth, levels
+        self.domain_bound = bool(domain_bound)
         self._zeros = None
 
     @classmethod
@@ -94,8 +126,14 @@ class KeyRegistry:
         return cls.from_leaves(pubkey_hashes(keys, n, k, device), depth, device)
 
     @classmethod
-    def from_leaves(cls, leaves, depth: int, device: int = 0) -> "KeyRegistry":
-        return cls(depth, merkle_levels(leaves, depth, device))
+    def build_domains(cls, pairs, depth: int, n: int = 121, k: int = 17, device: int = 0) -> "KeyRegistry":
+        """The domain-bound registry of (domain, key) pairs, in that order: what an app spec with "keyDomain" proves
+        against.  Domains are lowercased and lose a trailing dot; non-ASCII, empty and over-255-byte names are refused."""
+        return cls.from_leaves(domain_key_leaves(pairs, n, k, device), depth, device, domain_bound=True)
+
+    @classmethod
+    def from_leaves(cls, leaves, depth: int, device: int = 0, domain_bound: bool = False) -> "KeyRegistry":
+        return cls(depth, merkle_levels(leaves, depth, device), domain_bound)
 
     @property
     def root(self) -> int:
@@ -134,13 +172,20 @@ class KeyRegistry:
         return i, sib
 
     def to_json(self) -> str:
-        """The depth and the leaves; from_json rebuilds the tree on the GPU."""
-        return json.dumps({"depth": self.depth, "leaves": [str(x) for x in self.levels[0]]})
+        """The depth and the leaves (and "leaf": "domainKey" for a domain-bound registry); from_json rebuilds the tree
+        on the GPU."""
+        d = {"depth": self.depth, "leaves": [str(x) for x in self.levels[0]]}
+        if self.domain_bound:
+            d["leaf"] = "domainKey"
+        return json.dumps(d)
 
     @classmethod
     def from_json(cls, text: str, device: int = 0) -> "KeyRegistry":
         d = json.loads(text)
-        return cls.from_leaves([int(x) for x in d["leaves"]], int(d["depth"]), device)
+        leaf = d.get("leaf", "pubkeyHash")
+        if leaf not in ("pubkeyHash", "domainKey"):
+            raise ValueError(f'unknown registry leaf {leaf!r}: "pubkeyHash" or "domainKey"')
+        return cls.from_leaves([int(x) for x in d["leaves"]], int(d["depth"]), device, domain_bound=leaf == "domainKey")
 
 
-__all__ = ["KeyRegistry", "pubkey_hashes", "merkle_levels"]
+__all__ = ["KeyRegistry", "pubkey_hashes", "domain_key_leaves", "domain_key_leaf", "merkle_levels"]

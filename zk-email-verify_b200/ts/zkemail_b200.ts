@@ -25,6 +25,7 @@ const zke_agg_verify = lib.func('int zke_agg_verify(const char*, const char*, si
 const zke_poseidon_hash = lib.func('int zke_poseidon_hash(const uint8_t*, size_t, uint8_t*)');
 const zke_poseidon_batch = lib.func('int zke_poseidon_batch(const uint8_t*, uint32_t, size_t, int, uint8_t*, char*, size_t)');
 const zke_pubkey_hashes = lib.func('int zke_pubkey_hashes(const uint8_t*, size_t, uint32_t, uint32_t, uint32_t, int, uint8_t*, char*, size_t)');
+const zke_domain_key_leaves = lib.func('int zke_domain_key_leaves(const uint8_t*, size_t, uint32_t, uint32_t, uint32_t, const uint8_t*, int, uint8_t*, char*, size_t)');
 const zke_merkle_build = lib.func('int64_t zke_merkle_build(const uint8_t*, size_t, uint32_t, int, uint8_t*, size_t, char*, size_t)');
 
 const cstr = (b: Buffer) => b.toString('utf8', 0, b.indexOf(0));
@@ -189,6 +190,35 @@ export function pubkeyHashes(moduli: bigint[], n = 121, k = 17, device = 0): big
   if (zke_pubkey_hashes(Buffer.concat(moduli.map((m) => toLe(m, bytes))), moduli.length, bytes, n, k, device, out, err, err.length) !== 0)
     throw new Error(cstr(err));
   return moduli.map((_, i) => fromLe32(out, i));
+}
+/** A domain in canonical form: ASCII (A-labels for international names), lower case, no trailing dot, 1..255 bytes. */
+const canonicalDomain = (domain: string): Buffer => {
+  if (!/^[\x01-\x7f]*$/.test(domain)) throw new Error(`domain ${domain} is not ASCII: give an international name in its A-label (xn--) form`);
+  let d = domain.toLowerCase();
+  if (d.endsWith('.')) d = d.slice(0, -1);
+  if (d.length < 1 || d.length > 255) throw new Error(`domain ${d} has ${d.length} bytes; a domain has 1 to 255`);
+  return Buffer.from(d, 'ascii');
+};
+/** PoseidonModular(PackBytes(domain, 255)): one Poseidon(9), the domain half of a domain-bound registry leaf. */
+export function domainHash(domain: string): bigint {
+  const row = Buffer.alloc(255);
+  canonicalDomain(domain).copy(row);
+  return poseidon(Array.from({ length: 9 }, (_, i) => {
+    let x = 0n;
+    for (let j = 30; j >= 0; --j) x = (x << 8n) | BigInt(31 * i + j < 255 ? row[31 * i + j] : 0);
+    return x;
+  }));
+}
+/** Domain-bound leaves Poseidon(2)([domainHash(domain), pubkeyHash(modulus)]) of (domain, modulus) pairs on the GPU:
+ *  the leaves of a registry for specs with "keyDomain". */
+export function domainKeyLeaves(pairs: [string, bigint][], n = 121, k = 17, device = 0): bigint[] {
+  if (pairs.length === 0) return [];
+  const bytes = Math.ceil((n * k) / 8);
+  const rows = Buffer.concat(pairs.map(([d]) => { const row = Buffer.alloc(255); canonicalDomain(d).copy(row); return row; }));
+  const out = Buffer.alloc(32 * pairs.length), err = Buffer.alloc(4096);
+  if (zke_domain_key_leaves(Buffer.concat(pairs.map(([, m]) => toLe(m, bytes))), pairs.length, bytes, n, k, rows, device, out, err, err.length) !== 0)
+    throw new Error(cstr(err));
+  return pairs.map((_, i) => fromLe32(out, i));
 }
 /** Every level of the registry tree, leaves first, root last. */
 export function merkleBuild(leaves: bigint[], depth: number, device = 0): bigint[][] {
