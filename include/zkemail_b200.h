@@ -181,7 +181,23 @@ int zke_poseidon_hash(const uint8_t* inputs, size_t n, uint8_t* out);
  *   H(l, r) = Poseidon(2)([l, r]).  Level l holds ceil(count / 2^l) nodes, a missing right child at level l is
  *   zeros[l] (zeros[0] = 0, zeros[l + 1] = H(zeros[l], zeros[l])); levels are written one after the other from the
  *   leaves (level 0) to the root.  Returns the bytes written, the size needed when levels == NULL, -2 if cap is too small.
- * zke_registry_device_ms: device time of the calling thread's last successful call above (CUDA events around its kernels). */
+ * zke_registry_open: the tree of zke_merkle_build (same refusals and messages), kept resident on `device` for in-place
+ *   updates; NULL with a message in err on a refusal.  A handle is used by one host thread at a time.
+ * zke_registry_update: sets leaf indices[i] to leaves[i] for i < k.  An index below the count replaces a leaf (a leaf of
+ *   0 revokes it: zeros[0] = 0, so revoking the last leaves gives the root of the tree without them); indices at or above
+ *   the count append and must be exactly count .. count + a - 1, in any order.  Refuses a leaf not below r (naming its
+ *   position in the update), a duplicate index, a gap and a count above 2^depth, all before any device write: a
+ *   refused update leaves the tree unchanged.  Rehashes only the ancestors of the updated leaves, so every level equals
+ *   zke_merkle_build's over the resulting leaves.  k = 0 does nothing.  Returns 0.
+ * zke_registry_nodes: out[k][32] = node indices[i] of level levels[i] (level 0 = the leaves), zeros[level] past the
+ *   level's size; refuses level > depth and index >= 2^(depth - level).  Authentication paths are the nodes
+ *   (l, (i >> l) ^ 1) for l < depth.  Returns 0.
+ * zke_registry_levels: every level, in zke_merkle_build's layout and size rules (the size needed when out == NULL, -2
+ *   if cap is too small).
+ * zke_registry_count: the number of leaves (0 for NULL).  zke_registry_close frees the handle (NULL is ignored).
+ * zke_registry_device_ms: device time of the calling thread's last successful call above (CUDA events around its kernels,
+ *   around the copy for zke_registry_levels). */
+typedef struct zke_registry zke_registry;     /* a registry tree resident on one GPU */
 int zke_poseidon_batch(const uint8_t* inputs, uint32_t width, size_t count, int device, uint8_t* out, char* err, size_t errcap);
 int zke_pubkey_hashes(const uint8_t* moduli, size_t count, uint32_t modulus_bytes, uint32_t n, uint32_t k, int device,
                       uint8_t* out, char* err, size_t errcap);
@@ -189,6 +205,13 @@ int zke_domain_key_leaves(const uint8_t* moduli, size_t count, uint32_t modulus_
                           const uint8_t* domains, int device, uint8_t* out, char* err, size_t errcap);
 int64_t zke_merkle_build(const uint8_t* leaves, size_t count, uint32_t depth, int device, uint8_t* levels, size_t cap,
                          char* err, size_t errcap);
+zke_registry* zke_registry_open(const uint8_t* leaves, size_t count, uint32_t depth, int device, char* err, size_t errcap);
+int zke_registry_update(zke_registry* r, const uint64_t* indices, const uint8_t* leaves, size_t k, char* err, size_t errcap);
+int zke_registry_nodes(zke_registry* r, const uint32_t* levels, const uint64_t* indices, size_t k, uint8_t* out,
+                       char* err, size_t errcap);
+int64_t zke_registry_levels(zke_registry* r, uint8_t* out, size_t cap, char* err, size_t errcap);
+uint64_t zke_registry_count(const zke_registry* r);
+void zke_registry_close(zke_registry* r);
 double zke_registry_device_ms(void);
 
 

@@ -1,5 +1,5 @@
 // Batched Poseidon and the Merkle registry of DKIM keys (include/zkemail_b200.h: zke_poseidon_batch, zke_pubkey_hashes,
-// zke_domain_key_leaves, zke_merkle_build).
+// zke_domain_key_leaves, zke_merkle_build, and the resident registry zke_registry_*).
 //
 // One thread runs one Poseidon instance: the Merkle node hash (width 3) with its state in registers, the other widths
 // from one instantiation that takes the width at run time (its state in the thread's stack frame).  The round constants and the MDS matrix of the width come from
@@ -10,13 +10,16 @@
 // The Merkle tree (node H(l, r) = Poseidon(2)([l, r])) is built level by level on the device: one kernel hashes the
 // lowest FUSE_LEVELS levels of a 2^FUSE_LEVELS-leaf subtree per block, keeping each level in shared memory, and one launch
 // per higher level hashes the pairs of the level below.  A missing right child at level l is zeros[l], the root of an
-// empty subtree of height l (computed on the host: at most 32 hashes).
+// empty subtree of height l (computed on the host: at most 32 hashes).  A resident registry (zke_registry_open) keeps the
+// levels on the device and updates k leaves in place: one launch per level, one thread per changed node.
 #include "ff.cuh"
 #include "device_engine.cuh"
 #include "cuda_host.hpp"
 #include "gadgets.hpp"
 #include "../../include/zkemail_b200.h"
+#include <algorithm>
 #include <cstring>
+#include <memory>
 #include <stdexcept>
 #include <string>
 #include <vector>
@@ -293,6 +296,54 @@ merkle_level_kernel(uint8_t* __restrict__ levels, uint64_t below_off, uint64_t b
     fr_store(levels + 32 * (off + j), node_hash(left, right, sh, sh + (8 + r_p) * 3, r_p));
 }
 
+// In-place updates of a resident tree (zke_registry_update).  idx[0..k) are the updated leaf indices, sorted and
+// distinct.  level 0: leaf i goes to position idx[i]
+__global__ void __launch_bounds__(REG_THREADS)
+registry_scatter_kernel(uint8_t* __restrict__ levels, const uint64_t* __restrict__ idx, const uint8_t* __restrict__ leaves,
+                        uint64_t k) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= k) return;
+    const uint4* src = reinterpret_cast<const uint4*>(leaves + 32 * i);
+    uint4* dst = reinterpret_cast<uint4*>(levels + 32 * idx[i]);
+    dst[0] = src[0];
+    dst[1] = src[1];
+}
+
+// level l from level l - 1: thread i rehashes the ancestor p = idx[i] >> l unless thread i - 1 has the same one (the
+// indices are sorted, so equal ancestors are adjacent and this keeps exactly one thread per changed node).  A node that
+// appends bring into range at level l covers leaf p 2^l >= the old count, an appended index, so it is always rehashed
+// here; so is its parent once its right child comes into range.  That is what lets an update skip every other node.
+__global__ void __launch_bounds__(REG_THREADS)
+registry_update_level_kernel(uint8_t* __restrict__ levels, const uint64_t* __restrict__ idx, uint64_t k, int l,
+                             uint64_t below_off, uint64_t below_size, uint64_t off, const uint8_t* __restrict__ consts,
+                             int r_p, const uint8_t* __restrict__ zero_below) {
+    extern __shared__ uint4 smem[];
+    Fr* sh = reinterpret_cast<Fr*>(smem);
+    stage_constants(sh, consts, n_constants(3, r_p));
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= k) return;
+    const uint64_t p = idx[i] >> l;
+    if (i > 0 && (idx[i - 1] >> l) == p) return;
+    bool b = false;                                       // every value was checked below r on the host
+    const Fr left = fr_load(levels + 32 * (below_off + 2 * p), &b);
+    const Fr right = fr_load(2 * p + 1 < below_size ? levels + 32 * (below_off + 2 * p + 1) : zero_below, &b);
+    fr_store(levels + 32 * (off + p), node_hash(left, right, sh, sh + (8 + r_p) * 3, r_p));
+}
+
+// out[i] = node idx[i] of level lv[i], or zeros[lv[i]] past the level's size (authentication paths, the host mirror)
+__global__ void __launch_bounds__(REG_THREADS)
+registry_gather_kernel(const uint8_t* __restrict__ levels, LevelTable lt, const uint32_t* __restrict__ lv,
+                       const uint64_t* __restrict__ idx, uint64_t k, const uint8_t* __restrict__ zeros, uint8_t* __restrict__ out) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= k) return;
+    const uint32_t l = lv[i];
+    const uint64_t j = idx[i];
+    const uint4* src = reinterpret_cast<const uint4*>(j < lt.size[l] ? levels + 32 * (lt.off[l] + j) : zeros + 32 * l);
+    uint4* dst = reinterpret_cast<uint4*>(out + 32 * i);
+    dst[0] = src[0];
+    dst[1] = src[1];
+}
+
 }  // namespace dev
 }  // namespace zke
 
@@ -376,7 +427,101 @@ std::string domain_fault(const uint8_t* d) {
     return "";
 }
 
+// the refusals of zke_merkle_build and zke_registry_open
+void check_tree(const uint8_t* leaves, size_t count, uint32_t depth) {
+    if (!leaves) throw std::runtime_error("null argument");
+    if (depth < 1 || depth > 32) throw std::runtime_error("depth must be 1..32, not " + std::to_string(depth));
+    if (count == 0) throw std::runtime_error("count must be at least 1");
+    if ((uint64_t)count > (1ull << depth))
+        throw std::runtime_error("count " + std::to_string(count) + " does not fit a tree of depth " + std::to_string(depth));
+}
+
+// level l starts at the sum of the sizes of levels below it in a tree of `cap` leaves and holds ceil(count / 2^l) nodes
+dev::LevelTable level_table(uint64_t count, uint64_t cap, uint32_t depth, uint64_t* total) {
+    dev::LevelTable lt;
+    uint64_t pos = 0;
+    for (uint32_t l = 0; l <= depth; ++l) {
+        lt.off[l] = pos;
+        lt.size[l] = (count + (1ull << l) - 1) >> l;
+        pos += (cap + (1ull << l) - 1) >> l;
+    }
+    if (total) *total = pos;
+    return lt;
+}
+
+// zeros[l], the root of an empty subtree of height l, standard form
+std::vector<U256> zero_nodes(uint32_t depth) {
+    std::vector<U256> zeros(depth + 1);
+    zeros[0] = U256{{0, 0, 0, 0}};
+    Fr z = Fr::zero();
+    for (uint32_t l = 1; l <= depth; ++l) { z = gadgets::poseidon_hash({z, z}); zeros[l] = z.to_u256(); }
+    return zeros;
+}
+
+// levels 1..depth of the tree whose `count` leaves are on the device at lt.off[0]; refuses a leaf not below r, naming it
+// (the host copy `leaves` is searched: the fused kernel reports the first leaf of the block)
+void build_tree(uint8_t* d, const dev::LevelTable& lt, uint64_t count, uint32_t depth, const WidthConsts& C,
+                const uint8_t* zeros, const uint8_t* leaves) {
+    DevBuf bad;
+    bad_flag(bad);
+    const int L = depth < (uint32_t)dev::FUSE_LEVELS ? (int)depth : dev::FUSE_LEVELS;
+    const size_t smem = C.smem(), smem_fused = smem + 32ull * dev::REG_THREADS;
+    set_smem(dev::merkle_fused_kernel, smem_fused);
+    Timer tm;
+    dev::merkle_fused_kernel<<<(uint32_t)((count + (1ull << L) - 1) >> L), dev::REG_THREADS, smem_fused>>>(d, lt, L, C.buf.p, C.r_p, zeros, reinterpret_cast<uint32_t*>(bad.p));
+    ZKE_COUNT_LAUNCH(1);
+    CHECK_LAUNCH();
+    for (uint32_t l = (uint32_t)L + 1; l <= depth; ++l) {
+        dev::merkle_level_kernel<<<blocks_for(lt.size[l]), dev::REG_THREADS, smem>>>(d, lt.off[l - 1], lt.size[l - 1], lt.off[l],
+                                                                                   lt.size[l], C.buf.p, C.r_p, zeros + 32ull * (l - 1));
+        ZKE_COUNT_LAUNCH(1);
+        CHECK_LAUNCH();
+    }
+    tm.stop();
+    const uint32_t b = read_bad(bad);
+    if (b != dev::NO_BAD) {
+        for (uint64_t i = b; i < count; ++i) {
+            U256 x;
+            memcpy(x.v, leaves + 32 * i, 32);
+            if (u256_cmp(x, fr_params().p) >= 0) throw std::runtime_error("leaf " + std::to_string(i) + " is not below r");
+        }
+        throw std::runtime_error("a leaf is not below r");
+    }
+}
+
 }  // namespace
+
+// A tree resident on one device (zke_registry_open): the levels in one buffer laid out as level_table(count, cap),
+// where cap >= count leaves have room; appends past cap double it (at most 2^depth) and move each level's live prefix.
+struct zke_registry {
+    int device;
+    uint32_t depth;
+    uint64_t count = 0, cap = 0;
+    dev::LevelTable lt{};
+    DevBuf levels, zeros, io, out;          // io, out: upload and download staging of update / nodes
+    WidthConsts C{3};
+
+    zke_registry(int dv, uint32_t d) : device(dv), depth(d) { zeros.upload(zero_nodes(d)); }
+
+    // room for `need` leaves (need <= 2^depth), keeping every live node
+    void reserve(uint64_t need) {
+        if (need <= cap) return;
+        uint64_t c = cap ? cap : need;
+        while (c < need) c *= 2;
+        c = std::min<uint64_t>(c, 1ull << depth);
+        uint64_t total = 0;
+        const dev::LevelTable nt = level_table(count, c, depth, &total);
+        DevBuf nb;
+        nb.alloc(32 * total);
+        if (count)
+            for (uint32_t l = 0; l <= depth; ++l)
+                CUDA_OK(cudaMemcpy(nb.p + 32 * nt.off[l], levels.p + 32 * lt.off[l], 32 * lt.size[l], cudaMemcpyDeviceToDevice));
+        std::swap(levels.p, nb.p);
+        std::swap(levels.bytes, nb.bytes);
+        lt = nt;
+        cap = c;
+    }
+};
 
 extern "C" {
 
@@ -476,59 +621,154 @@ int zke_domain_key_leaves(const uint8_t* moduli, size_t count, uint32_t modulus_
 int64_t zke_merkle_build(const uint8_t* leaves, size_t count, uint32_t depth, int device, uint8_t* levels, size_t cap,
                          char* err, size_t errcap) {
     try {
-        if (!leaves) throw std::runtime_error("null argument");
-        if (depth < 1 || depth > 32) throw std::runtime_error("depth must be 1..32, not " + std::to_string(depth));
-        if (count == 0) throw std::runtime_error("count must be at least 1");
-        if ((uint64_t)count > (1ull << depth))
-            throw std::runtime_error("count " + std::to_string(count) + " does not fit a tree of depth " + std::to_string(depth));
-        dev::LevelTable lt;
+        check_tree(leaves, count, depth);
         uint64_t total = 0;
-        for (uint32_t l = 0; l <= depth; ++l) {
-            lt.off[l] = total;
-            lt.size[l] = (count + (1ull << l) - 1) >> l;
-            total += lt.size[l];
-        }
+        const dev::LevelTable lt = level_table(count, count, depth, &total);
         const int64_t bytes = (int64_t)(32 * total);
         if (!levels) return bytes;
         if (cap < (size_t)bytes) return -2;
         select_device(device);
-        std::vector<U256> zeros(depth + 1);
-        zeros[0] = U256{{0, 0, 0, 0}};
-        Fr z = Fr::zero();
-        for (uint32_t l = 1; l <= depth; ++l) { z = gadgets::poseidon_hash({z, z}); zeros[l] = z.to_u256(); }
         WidthConsts C(3);
-        DevBuf d, dz, bad;
-        bad_flag(bad);
-        dz.upload(zeros);
+        DevBuf d, dz;
+        dz.upload(zero_nodes(depth));
         d.alloc((size_t)bytes);
         CUDA_OK(cudaMemcpy(d.p, leaves, 32ull * count, cudaMemcpyHostToDevice));
-        const int L = depth < (uint32_t)dev::FUSE_LEVELS ? (int)depth : dev::FUSE_LEVELS;
-        const size_t smem = C.smem(), smem_fused = smem + 32ull * dev::REG_THREADS;
-        set_smem(dev::merkle_fused_kernel, smem_fused);
+        build_tree(d.p, lt, count, depth, C, dz.p, leaves);
+        CUDA_OK(cudaMemcpy(levels, d.p, (size_t)bytes, cudaMemcpyDeviceToHost));
+        return bytes;
+    } catch (const std::exception& e) { set_err(err, errcap, e.what()); return -1; }
+}
+
+zke_registry* zke_registry_open(const uint8_t* leaves, size_t count, uint32_t depth, int device, char* err, size_t errcap) {
+    try {
+        check_tree(leaves, count, depth);
+        select_device(device);
+        std::unique_ptr<zke_registry> r(new zke_registry(device, depth));
+        r->reserve(count);
+        r->count = count;
+        r->lt = level_table(count, r->cap, depth, nullptr);
+        CUDA_OK(cudaMemcpy(r->levels.p, leaves, 32ull * count, cudaMemcpyHostToDevice));
+        build_tree(r->levels.p, r->lt, count, depth, r->C, r->zeros.p, leaves);
+        return r.release();
+    } catch (const std::exception& e) { set_err(err, errcap, e.what()); return nullptr; }
+}
+
+int zke_registry_update(zke_registry* r, const uint64_t* indices, const uint8_t* leaves, size_t k, char* err, size_t errcap) {
+    try {
+        if (!r) throw std::runtime_error("null registry");
+        if (k == 0) return 0;
+        if (!indices || !leaves) throw std::runtime_error("null argument");
+        // every check before the first device write: a refused update leaves the tree as it was
+        for (size_t i = 0; i < k; ++i) {
+            U256 x;
+            memcpy(x.v, leaves + 32 * i, 32);
+            if (u256_cmp(x, fr_params().p) >= 0)
+                throw std::runtime_error("leaf " + std::to_string(i) + " of the update is not below r");
+        }
+        std::vector<size_t> ord(k);
+        for (size_t i = 0; i < k; ++i) ord[i] = i;
+        std::sort(ord.begin(), ord.end(), [&](size_t a, size_t b) { return indices[a] < indices[b]; });
+        uint64_t appended = 0;
+        for (size_t j = 0; j < k; ++j) {
+            const uint64_t x = indices[ord[j]];
+            if (j > 0 && x == indices[ord[j - 1]]) throw std::runtime_error("index " + std::to_string(x) + " appears twice");
+            if (x >= r->count) {
+                if (x != r->count + appended)
+                    throw std::runtime_error("index " + std::to_string(x) + " leaves a gap after the " +
+                                             std::to_string(r->count + appended) + " leaves");
+                ++appended;
+            }
+        }
+        const uint64_t count = r->count + appended;
+        if (count > (1ull << r->depth))
+            throw std::runtime_error(std::to_string(count) + " leaves do not fit a tree of depth " + std::to_string(r->depth));
+        // one upload: the leaves in index order, then the sorted indices
+        std::vector<uint8_t> host(40 * k);
+        uint64_t* idx = reinterpret_cast<uint64_t*>(host.data() + 32 * k);
+        for (size_t j = 0; j < k; ++j) {
+            memcpy(host.data() + 32 * j, leaves + 32 * ord[j], 32);
+            idx[j] = indices[ord[j]];
+        }
+        CUDA_OK(cudaSetDevice(r->device));
+        r->reserve(count);
+        r->count = count;
+        r->lt = level_table(count, r->cap, r->depth, nullptr);
+        r->io.reserve(host.size());
+        CUDA_OK(cudaMemcpy(r->io.p, host.data(), host.size(), cudaMemcpyHostToDevice));
+        const uint64_t* didx = reinterpret_cast<const uint64_t*>(r->io.p + 32 * k);
+        const dev::LevelTable& lt = r->lt;
         Timer tm;
-        dev::merkle_fused_kernel<<<(uint32_t)((count + (1ull << L) - 1) >> L), dev::REG_THREADS, smem_fused>>>(d.p, lt, L, C.buf.p, C.r_p, dz.p, reinterpret_cast<uint32_t*>(bad.p));
+        dev::registry_scatter_kernel<<<blocks_for(k), dev::REG_THREADS>>>(r->levels.p + 32 * lt.off[0], didx, r->io.p, k);
         ZKE_COUNT_LAUNCH(1);
         CHECK_LAUNCH();
-        for (uint32_t l = (uint32_t)L + 1; l <= depth; ++l) {
-            dev::merkle_level_kernel<<<blocks_for(lt.size[l]), dev::REG_THREADS, smem>>>(d.p, lt.off[l - 1], lt.size[l - 1], lt.off[l],
-                                                                                       lt.size[l], C.buf.p, C.r_p, dz.p + 32ull * (l - 1));
+        for (uint32_t l = 1; l <= r->depth; ++l) {
+            dev::registry_update_level_kernel<<<blocks_for(k), dev::REG_THREADS, r->C.smem()>>>(
+                r->levels.p, didx, k, (int)l, lt.off[l - 1], lt.size[l - 1], lt.off[l], r->C.buf.p, r->C.r_p,
+                r->zeros.p + 32ull * (l - 1));
             ZKE_COUNT_LAUNCH(1);
             CHECK_LAUNCH();
         }
         tm.stop();
-        const uint32_t b = read_bad(bad);
-        if (b != dev::NO_BAD) {
-            // the fused kernel reports the first leaf of the block: find the leaf on the host
-            for (uint64_t i = b; i < count; ++i) {
-                U256 x;
-                memcpy(x.v, leaves + 32 * i, 32);
-                if (u256_cmp(x, fr_params().p) >= 0) throw std::runtime_error("leaf " + std::to_string(i) + " is not below r");
-            }
-            throw std::runtime_error("a leaf is not below r");
+        return 0;
+    } catch (const std::exception& e) { set_err(err, errcap, e.what()); return -1; }
+}
+
+int zke_registry_nodes(zke_registry* r, const uint32_t* levels, const uint64_t* indices, size_t k, uint8_t* out,
+                       char* err, size_t errcap) {
+    try {
+        if (!r) throw std::runtime_error("null registry");
+        if (k == 0) return 0;
+        if (!levels || !indices || !out) throw std::runtime_error("null argument");
+        for (size_t i = 0; i < k; ++i) {
+            if (levels[i] > r->depth)
+                throw std::runtime_error("node " + std::to_string(i) + ": level " + std::to_string(levels[i]) +
+                                         " is above the root (level " + std::to_string(r->depth) + ")");
+            if (indices[i] >= (1ull << (r->depth - levels[i])))
+                throw std::runtime_error("node " + std::to_string(i) + ": index " + std::to_string(indices[i]) +
+                                         " is outside level " + std::to_string(levels[i]) + " of a tree of depth " +
+                                         std::to_string(r->depth));
         }
-        CUDA_OK(cudaMemcpy(levels, d.p, (size_t)bytes, cudaMemcpyDeviceToHost));
+        CUDA_OK(cudaSetDevice(r->device));
+        r->io.reserve(12 * k);
+        CUDA_OK(cudaMemcpy(r->io.p, indices, 8 * k, cudaMemcpyHostToDevice));
+        CUDA_OK(cudaMemcpy(r->io.p + 8 * k, levels, 4 * k, cudaMemcpyHostToDevice));
+        r->out.reserve(32 * k);
+        Timer tm;
+        dev::registry_gather_kernel<<<blocks_for(k), dev::REG_THREADS>>>(
+            r->levels.p, r->lt, reinterpret_cast<const uint32_t*>(r->io.p + 8 * k), reinterpret_cast<const uint64_t*>(r->io.p),
+            k, r->zeros.p, r->out.p);
+        ZKE_COUNT_LAUNCH(1);
+        CHECK_LAUNCH();
+        tm.stop();
+        CUDA_OK(cudaMemcpy(out, r->out.p, 32 * k, cudaMemcpyDeviceToHost));
+        return 0;
+    } catch (const std::exception& e) { set_err(err, errcap, e.what()); return -1; }
+}
+
+int64_t zke_registry_levels(zke_registry* r, uint8_t* out, size_t cap, char* err, size_t errcap) {
+    try {
+        if (!r) throw std::runtime_error("null registry");
+        uint64_t total = 0;
+        for (uint32_t l = 0; l <= r->depth; ++l) total += r->lt.size[l];
+        const int64_t bytes = (int64_t)(32 * total);
+        if (!out) return bytes;
+        if (cap < (size_t)bytes) return -2;
+        CUDA_OK(cudaSetDevice(r->device));
+        Timer tm;
+        uint64_t pos = 0;
+        for (uint32_t l = 0; l <= r->depth; pos += r->lt.size[l], ++l)
+            CUDA_OK(cudaMemcpy(out + 32ull * pos, r->levels.p + 32 * r->lt.off[l], 32 * r->lt.size[l], cudaMemcpyDeviceToHost));
+        tm.stop();
         return bytes;
     } catch (const std::exception& e) { set_err(err, errcap, e.what()); return -1; }
+}
+
+uint64_t zke_registry_count(const zke_registry* r) { return r ? r->count : 0; }
+
+void zke_registry_close(zke_registry* r) {
+    if (!r) return;
+    cudaSetDevice(r->device);
+    delete r;
 }
 
 double zke_registry_device_ms(void) { return g_last_device_ms; }

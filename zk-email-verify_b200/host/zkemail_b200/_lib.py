@@ -63,6 +63,12 @@ zke_pubkey_hashes = _sig("zke_pubkey_hashes", c_int, [c_char_p, c_size_t, c_u32,
 zke_domain_key_leaves = _sig("zke_domain_key_leaves", c_int, [c_char_p, c_size_t, c_u32, c_u32, c_u32, c_char_p, c_int, c_void_p,
                                                                c_char_p, c_size_t])
 zke_merkle_build = _sig("zke_merkle_build", c_i64, [c_char_p, c_size_t, c_u32, c_int, c_void_p, c_size_t, c_char_p, c_size_t])
+zke_registry_open = _sig("zke_registry_open", c_void_p, [c_char_p, c_size_t, c_u32, c_int, c_char_p, c_size_t])
+zke_registry_update = _sig("zke_registry_update", c_int, [c_void_p, c_void_p, c_char_p, c_size_t, c_char_p, c_size_t])
+zke_registry_nodes = _sig("zke_registry_nodes", c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, c_char_p, c_size_t])
+zke_registry_levels = _sig("zke_registry_levels", c_i64, [c_void_p, c_void_p, c_size_t, c_char_p, c_size_t])
+zke_registry_count = _sig("zke_registry_count", c_u64, [c_void_p])
+zke_registry_close = _sig("zke_registry_close", None, [c_void_p])
 zke_registry_device_ms = _sig("zke_registry_device_ms", ctypes.c_double, [])
 zke_device_count = _sig("zke_device_count", c_int, [])
 zke_version = _sig("zke_version", c_char_p, [])

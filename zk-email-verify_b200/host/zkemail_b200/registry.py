@@ -4,7 +4,8 @@ A leaf is a key's pubkeyHash - poseidon_large(modulus, ceil(k / 2), 2n), what Em
 H(l, r) = Poseidon(2)([l, r]).  With m leaves and depth d, positions m .. 2^d - 1 hold 0: level l stores ceil(m / 2^l)
 nodes, a missing right child at level l is zeros[l] (zeros[0] = 0, zeros[l + 1] = H(zeros[l], zeros[l])), and the root is
 level d's single node.  Bit l of a leaf's index is 1 when its ancestor at level l is a right child.  The leaves and the
-tree are computed on the GPU (zke_pubkey_hashes, zke_merkle_build).
+tree are computed on the GPU (zke_pubkey_hashes, zke_merkle_build), and KeyRegistry.update / append change leaves in
+place there (zke_registry_update), rehashing only the ancestors of the changed leaves.
 
 The root says "signed by some key in this set" and nothing about which key, so nothing about which domain: a verifier
 compares a proof's registryRoot with the root of the registry it trusts.
@@ -16,6 +17,7 @@ lists for the domain the proof names".  One key may sit under several domains an
 from __future__ import annotations
 import base64
 import ctypes
+from array import array
 import json
 import re
 
@@ -86,27 +88,69 @@ def domain_key_leaf(domain, key, n: int = 121, k: int = 17) -> int:
 def merkle_levels(leaves, depth: int, device: int = 0) -> list[list[int]]:
     """Every level of the tree over `leaves` (level 0 = the leaves, the last level = [root]), built on the GPU."""
     leaves = [int(x) for x in leaves]
-    data = b"".join(x.to_bytes(32, "little") if 0 <= x < FR_MODULUS else b"\xff" * 32 for x in leaves)
     err = ctypes.create_string_buffer(L.ERRCAP)
+    data = _leaf_image(leaves)
     need = L.zke_merkle_build(data, len(leaves), depth, device, None, 0, err, L.ERRCAP)
     if need < 0:
         raise L.ZkeError(err.value.decode())
     buf = ctypes.create_string_buffer(need)
     if L.zke_merkle_build(data, len(leaves), depth, device, buf, need, err, L.ERRCAP) != need:
         raise L.ZkeError(err.value.decode())
-    flat, levels, pos, m = _ints(buf.raw, need // 32), [], 0, len(leaves)
+    return _split_levels(buf.raw, len(leaves), depth)
+
+
+def _leaf_image(leaves) -> bytes:
+    """32-byte little-endian leaves; a value outside [0, r) becomes 2^256 - 1, which the library refuses by position."""
+    return b"".join(x.to_bytes(32, "little") if 0 <= x < FR_MODULUS else b"\xff" * 32 for x in leaves)
+
+
+def _split_levels(raw: bytes, count: int, depth: int) -> list[list[int]]:
+    """The levels of a tree over `count` leaves from zke_merkle_build's (and zke_registry_levels') flat layout."""
+    flat, levels, pos = _ints(raw, len(raw) // 32), [], 0
     for lvl in range(depth + 1):
-        size = -(-m // (1 << lvl))
+        size = -(-count // (1 << lvl))
         levels.append(flat[pos:pos + size])
         pos += size
     return levels
 
 
+def _check_update(changes, count: int, depth: int) -> list[tuple[int, int]]:
+    """The (index, leaf) pairs of an update of a tree of `count` leaves and depth `depth`, validated as
+    zke_registry_update validates them: each leaf below r (named by its position in the update), no index twice, the
+    indices at or above `count` exactly count, count + 1, ... in any order, and at most 2^depth leaves after."""
+    pairs = list(changes.items()) if isinstance(changes, dict) else list(changes)
+    out = []
+    for pos, pair in enumerate(pairs):
+        index, leaf = (int(x) for x in pair)
+        if index < 0:
+            raise ValueError(f"index {index} of the update is negative")
+        if not 0 <= leaf < FR_MODULUS:
+            raise ValueError(f"leaf {pos} of the update is not below r")
+        out.append((index, leaf))
+    indices = sorted(i for i, _ in out)
+    appended = 0
+    for j, i in enumerate(indices):
+        if j and i == indices[j - 1]:
+            raise ValueError(f"index {i} appears twice")
+        if i >= count:
+            if i != count + appended:
+                raise ValueError(f"index {i} leaves a gap after the {count + appended} leaves")
+            appended += 1
+    if count + appended > 1 << depth:
+        raise ValueError(f"{count + appended} leaves do not fit a tree of depth {depth}")
+    return out
+
+
 class KeyRegistry:
     """A registry of DKIM keys: depth d, the levels of its tree.  build(), build_domains() and from_leaves() compute them on
-    the GPU; the constructor only checks shapes.  domain_bound: the leaves are (domain, key) leaves (build_domains)."""
+    the GPU; the constructor only checks shapes.  domain_bound: the leaves are (domain, key) leaves (build_domains).
 
-    def __init__(self, depth: int, levels, domain_bound: bool = False):
+    update() and append() change leaves in place: on first use they open a copy of the tree resident on `device`
+    (zke_registry_open), rehash only the ancestors of the changed leaves there, and patch `levels` with the nodes that
+    changed, so root, path, index_of and to_json follow.  Change `levels` only through these methods: the resident tree
+    is not read back.  close() (also on garbage collection) frees it; a registry is used by one thread at a time."""
+
+    def __init__(self, depth: int, levels, domain_bound: bool = False, device: int = 0):
         if not isinstance(depth, int) or not 1 <= depth <= 32:
             raise ValueError(f"depth must be 1..32, not {depth!r}")
         levels = [[int(x) for x in lvl] for lvl in levels]
@@ -118,7 +162,9 @@ class KeyRegistry:
                 raise ValueError(f"level {lvl} holds {len(nodes)} nodes, not ceil({m} / 2^{lvl})")
         self.depth, self.levels = depth, levels
         self.domain_bound = bool(domain_bound)
+        self.device = device
         self._zeros = None
+        self._h = None
 
     @classmethod
     def build(cls, keys, depth: int, n: int = 121, k: int = 17, device: int = 0) -> "KeyRegistry":
@@ -133,7 +179,73 @@ class KeyRegistry:
 
     @classmethod
     def from_leaves(cls, leaves, depth: int, device: int = 0, domain_bound: bool = False) -> "KeyRegistry":
-        return cls(depth, merkle_levels(leaves, depth, device), domain_bound)
+        return cls(depth, merkle_levels(leaves, depth, device), domain_bound, device)
+
+    def update(self, changes) -> None:
+        """Set leaves: `changes` is a dict or an iterable of (index, leaf) pairs, leaves as field elements (pubkey_hashes,
+        domain_key_leaves).  An index below the count replaces that leaf; a leaf of 0 revokes it, and since zeros[0] = 0,
+        revoking the last leaves gives the root of the registry without them.  Indices from the count on append and
+        must be exactly count, count + 1, ... in any order.  Refused with ValueError, before anything changes: a leaf not
+        below r, an index given twice, a gap after the last leaf, more than 2^depth leaves."""
+        pairs = _check_update(changes, len(self.levels[0]), self.depth)
+        if not pairs:
+            return
+        h = self._handle()
+        err = ctypes.create_string_buffer(L.ERRCAP)
+        if L.zke_registry_update(h, array("Q", (i for i, _ in pairs)).tobytes(), b"".join(x.to_bytes(32, "little") for _, x in pairs),
+                                 len(pairs), err, L.ERRCAP) != 0:
+            raise L.ZkeError(err.value.decode())
+        self._mirror(pairs)
+
+    def append(self, leaves) -> list[int]:
+        """Append leaves (field elements) after the last one; returns their indices."""
+        first = len(self.levels[0])
+        leaves = list(leaves)
+        self.update(zip(range(first, first + len(leaves)), leaves))
+        return list(range(first, first + len(leaves)))
+
+    def close(self) -> None:
+        """Free the resident tree, if one was opened; a later update opens it again from `levels`."""
+        h, self._h = getattr(self, "_h", None), None
+        if h:
+            L.zke_registry_close(h)
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def __getstate__(self):
+        return dict(self.__dict__, _h=None)        # a copy opens a resident tree of its own
+
+    def _handle(self):
+        if self._h is None:
+            err = ctypes.create_string_buffer(L.ERRCAP)
+            h = L.zke_registry_open(_leaf_image(self.levels[0]), len(self.levels[0]), self.depth, self.device, err, L.ERRCAP)
+            if not h:
+                raise L.ZkeError(err.value.decode())
+            self._h = h
+        return self._h
+
+    def _mirror(self, pairs) -> None:
+        """Patch `levels` after an update of `pairs` on the device: the ancestors of the changed leaves, fetched with one
+        zke_registry_nodes call (new nodes from appends are all among them)."""
+        count = max(len(self.levels[0]), max(i for i, _ in pairs) + 1)
+        for lvl, nodes in enumerate(self.levels):
+            nodes.extend([0] * (-(-count // (1 << lvl)) - len(nodes)))
+        for i, x in pairs:
+            self.levels[0][i] = x
+        changed, lv, ix = sorted(i for i, _ in pairs), [], []
+        for lvl in range(1, self.depth + 1):
+            changed = sorted({j >> 1 for j in changed})
+            lv += [lvl] * len(changed)
+            ix += changed
+        out, err = ctypes.create_string_buffer(32 * len(ix)), ctypes.create_string_buffer(L.ERRCAP)
+        if L.zke_registry_nodes(self._h, array("I", lv).tobytes(), array("Q", ix).tobytes(), len(ix), out, err, L.ERRCAP) != 0:
+            raise L.ZkeError(err.value.decode())
+        for lvl, j, x in zip(lv, ix, _ints(out.raw, len(ix))):
+            self.levels[lvl][j] = x
 
     @property
     def root(self) -> int:

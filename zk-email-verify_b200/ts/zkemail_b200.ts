@@ -27,6 +27,11 @@ const zke_poseidon_batch = lib.func('int zke_poseidon_batch(const uint8_t*, uint
 const zke_pubkey_hashes = lib.func('int zke_pubkey_hashes(const uint8_t*, size_t, uint32_t, uint32_t, uint32_t, int, uint8_t*, char*, size_t)');
 const zke_domain_key_leaves = lib.func('int zke_domain_key_leaves(const uint8_t*, size_t, uint32_t, uint32_t, uint32_t, const uint8_t*, int, uint8_t*, char*, size_t)');
 const zke_merkle_build = lib.func('int64_t zke_merkle_build(const uint8_t*, size_t, uint32_t, int, uint8_t*, size_t, char*, size_t)');
+const zke_registry_open = lib.func('void* zke_registry_open(const uint8_t*, size_t, uint32_t, int, char*, size_t)');
+const zke_registry_update = lib.func('int zke_registry_update(void*, const uint64_t*, const uint8_t*, size_t, char*, size_t)');
+const zke_registry_nodes = lib.func('int zke_registry_nodes(void*, const uint32_t*, const uint64_t*, size_t, uint8_t*, char*, size_t)');
+const zke_registry_count = lib.func('uint64_t zke_registry_count(void*)');
+const zke_registry_close = lib.func('void zke_registry_close(void*)');
 
 const cstr = (b: Buffer) => b.toString('utf8', 0, b.indexOf(0));
 type Entry = { circuit: unknown; zkey: unknown; ctx: unknown };
@@ -234,4 +239,44 @@ export function merkleBuild(leaves: bigint[], depth: number, device = 0): bigint
     pos += size;
   }
   return levels;
+}
+
+/** A registry tree resident on one GPU (zke_registry_*), updated in place: only the ancestors of changed leaves are
+ *  rehashed.  Leaves are field elements (pubkeyHashes, domainKeyLeaves).  One caller at a time; close() frees it. */
+export class Registry {
+  private h: unknown;
+  constructor(leaves: bigint[], readonly depth: number, device = 0) {
+    const err = Buffer.alloc(4096);
+    this.h = zke_registry_open(Buffer.concat(leaves.map((x) => toLe(x, 32))), leaves.length, depth, device, err, err.length);
+    if (!this.h) throw new Error(cstr(err));
+  }
+  get count(): number { return Number(zke_registry_count(this.h)); }
+  /** Replace (leaf 0 revokes) and append: indices from `count` on must be count, count + 1, ... in any order. */
+  update(changes: [number, bigint][]): void {
+    if (changes.length === 0) return;
+    const err = Buffer.alloc(4096);
+    const rc = zke_registry_update(this.h, BigUint64Array.from(changes.map(([i]) => BigInt(i))),
+      Buffer.concat(changes.map(([, x]) => toLe(x, 32))), changes.length, err, err.length);
+    if (rc !== 0) throw new Error(cstr(err));
+  }
+  /** Appends after the last leaf; returns the new indices. */
+  append(leaves: bigint[]): number[] {
+    const first = this.count, idx = leaves.map((_, j) => first + j);
+    this.update(idx.map((i, j) => [i, leaves[j]]));
+    return idx;
+  }
+  private nodes(levels: number[], indices: number[]): bigint[] {
+    const out = Buffer.alloc(32 * levels.length), err = Buffer.alloc(4096);
+    if (zke_registry_nodes(this.h, Uint32Array.from(levels), BigUint64Array.from(indices.map(BigInt)), levels.length, out, err, err.length) !== 0)
+      throw new Error(cstr(err));
+    return levels.map((_, i) => fromLe32(out, i));
+  }
+  /** The circuit's registryIndex and registrySiblings for leaf i. */
+  path(i: number): { index: number; siblings: bigint[] } {
+    if (!(i >= 0 && i < this.count)) throw new Error(`leaf ${i} is not in a registry of ${this.count} keys`);
+    const levels = Array.from({ length: this.depth }, (_, l) => l);
+    return { index: i, siblings: this.nodes(levels, levels.map((l) => Number((BigInt(i) >> BigInt(l)) ^ 1n))) };
+  }
+  get root(): bigint { return this.nodes([this.depth], [0])[0]; }
+  close(): void { if (this.h) zke_registry_close(this.h); this.h = null; }
 }
