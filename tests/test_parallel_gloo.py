@@ -108,8 +108,8 @@ def test_shard_exchange_moves_columns_to_rows_and_back():
 
 
 def _combine_worker(rank, world, port, q):
-    """Each rank sums its share of the five multi-exponentiations with the Python oracle's curve arithmetic, the partial
-    points are all-gathered over gloo and combined by the product's host routine (zke_shard_combine_raw)."""
+    """Each rank sums its share of the five multi-exponentiations with the Python oracle's curve arithmetic (the shares of
+    the engine's column layout, tests/test_shard_partials_host.py), the partial points are all-gathered over gloo and combined by the product's host routine (zke_shard_combine_raw)."""
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     for p in (root, os.path.join(root, "zk-email-verify_b200", "host"), os.path.join(root, "tests")):
         sys.path.insert(0, p)
@@ -119,7 +119,7 @@ def _combine_worker(rank, world, port, q):
     import zkemail_b200 as z
     from zkemail_b200 import _lib as L
     from zkemail_b200 import iden3_binfile as B
-    from zkemail_b200.parallel import shard_range
+    from test_shard_partials_host import column_positions, point_range
     from zkutil import oracle_setup, oracle_prove, oracle_witness
     from oracle import bn254
     os.environ["MASTER_ADDR"] = "127.0.0.1"
@@ -160,7 +160,8 @@ def _combine_worker(rank, world, port, q):
             if p is not None and scalars[i]:
                 acc = bn254.g1_add(acc, bn254.g1_mul(p, scalars[i]))
         return acc
-    mine_pts, mine_h = shard_range(m, rank, world), shard_range(n, rank, world)
+    # the engine's shares (zke_shard_end): a contiguous point range, and for H the rank's columns of every block
+    mine_pts, mine_h = point_range(m, rank, world), [int(i) for i in column_positions(n, rank, world)]
     pa, pb1, pc, ph = msm1("A", vals, mine_pts), msm1("B1", vals, mine_pts), msm1("C", vals, mine_pts), msm1("H", d, mine_h)
     pb2 = None
     for i in mine_pts:
