@@ -148,7 +148,6 @@ G1AffineH g1_mont_at(const uint8_t* p) { return G1AffineH{fq_mont_at(p), fq_mont
 G2AffineH g2_mont_at(const uint8_t* p) {
     return G2AffineH{Fq2{fq_mont_at(p), fq_mont_at(p + 32)}, Fq2{fq_mont_at(p + 64), fq_mont_at(p + 96)}};
 }
-void fr_bytes(const Fr& x, uint8_t* out) { const U256 s = x.to_u256(); memcpy(out, s.v, 32); }
 
 // Per-call device state of one aggregation
 struct AggRun {
@@ -198,7 +197,7 @@ struct AggRun {
     template <class F>
     void scale(uint8_t* pts, const std::vector<Fr>& s) {
         std::vector<uint8_t> b(32 * s.size());
-        for (size_t i = 0; i < s.size(); ++i) fr_bytes(s[i], &b[32 * i]);
+        for (size_t i = 0; i < s.size(); ++i) store_fr(&b[32 * i], s[i]);
         uint8_t* d = scal.reserve(b.size());
         CUDA_OK(cudaMemcpyAsync(d, b.data(), b.size(), cudaMemcpyHostToDevice, st));
         dev::agg_scale_kernel<F><<<agg_blocks(s.size()), dev::AGG_THREADS, 0, st>>>(pts, d, (uint32_t)s.size());
@@ -218,7 +217,7 @@ struct AggRun {
     AffineH<F> msm(const uint8_t* points, const std::vector<Fr>& s) {
         const uint32_t n = (uint32_t)s.size();
         std::vector<uint8_t> b(32 * s.size());
-        for (size_t i = 0; i < s.size(); ++i) fr_bytes(s[i], &b[32 * i]);
+        for (size_t i = 0; i < s.size(); ++i) store_fr(&b[32 * i], s[i]);
         DevBuf d_s, ws, res;
         CUDA_OK(cudaMemcpyAsync(d_s.reserve(b.size()), b.data(), b.size(), cudaMemcpyHostToDevice, st));
         typedef typename std::conditional<sizeof(F) == sizeof(Fq), dev::Fq, dev::Fq2>::type DF;
@@ -236,13 +235,8 @@ struct AggRun {
     ~AggRun() { if (st) cudaStreamDestroy(st); }
 };
 
-template <class P>
-void put_point(uint8_t*& o, const P& p) {
-    std::vector<uint8_t> b;
-    if constexpr (sizeof(p.x) == sizeof(Fq)) agg::put_g1(b, p); else agg::put_g2(b, p);
-    memcpy(o, b.data(), b.size());
-    o += b.size();
-}
+void put_point(uint8_t*& o, const G1AffineH& p) { store_g1(o, p); o += agg::G1_BYTES; }
+void put_point(uint8_t*& o, const G2AffineH& p) { store_g2(o, p); o += agg::G2_BYTES; }
 
 std::vector<Fr> powers(const Fr& x, size_t n) {
     std::vector<Fr> p(n);

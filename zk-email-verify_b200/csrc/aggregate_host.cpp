@@ -81,28 +81,18 @@ void check_count(size_t n) {
         throw std::runtime_error("the number of proofs must be a power of two from 2 to 8192, not " + std::to_string(n));
 }
 
-void put_fq(std::vector<uint8_t>& out, const Fq& x) { const U256 s = x.to_u256(); const uint8_t* b = (const uint8_t*)s.v; out.insert(out.end(), b, b + 32); }
-void put_fr(std::vector<uint8_t>& out, const Fr& x) { const U256 s = x.to_u256(); const uint8_t* b = (const uint8_t*)s.v; out.insert(out.end(), b, b + 32); }
-void put_g1(std::vector<uint8_t>& out, const G1AffineH& p) { put_fq(out, p.x); put_fq(out, p.y); }
-void put_g2(std::vector<uint8_t>& out, const G2AffineH& p) { put_fq(out, p.x.c0); put_fq(out, p.x.c1); put_fq(out, p.y.c0); put_fq(out, p.y.c1); }
 void put_vkey(std::vector<uint8_t>& out, const VerifyingKey& vk) {
     put_g1(out, vk.alpha1); put_g2(out, vk.beta2); put_g2(out, vk.gamma2); put_g2(out, vk.delta2);
     for (auto& p : vk.ic) put_g1(out, p);
 }
 
-Fq fq_at(const uint8_t* p) {
-    U256 x;
-    memcpy(x.v, p, 32);
-    if (u256_cmp(x, fq_params().p) >= 0) throw std::runtime_error("coordinate not reduced");
-    return Fq::from_u256(x);
-}
 G1AffineH g1_at(const uint8_t* p) {
-    const G1AffineH a{fq_at(p), fq_at(p + 32)};
+    const G1AffineH a = load_g1(p);
     if (!g1_on_curve(a)) throw std::runtime_error("G1 point not on the curve");
     return a;
 }
 G2AffineH g2_at(const uint8_t* p) {
-    const G2AffineH a{Fq2{fq_at(p), fq_at(p + 32)}, Fq2{fq_at(p + 64), fq_at(p + 96)}};
+    const G2AffineH a = load_g2(p);
     if (!g2_on_curve(a)) throw std::runtime_error("G2 point not on the twist curve");
     if (!g2_in_subgroup(a)) throw std::runtime_error("G2 point not in the order-r subgroup");
     return a;

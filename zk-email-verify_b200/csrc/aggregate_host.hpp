@@ -34,16 +34,10 @@ Fr challenge(const std::vector<uint8_t>& bytes);
 // r = H(tag, Groth16 key, n as u32, T_AB U_AB T_C U_C, public signals); every later challenge H(previous, messages)
 Fr first_challenge(const VerifyingKey& vk, size_t n, const uint8_t* com, const uint8_t* publics);
 Fr next_challenge(const Fr& prev, const uint8_t* msg, size_t len);
-void put_fq(std::vector<uint8_t>& out, const Fq& x);
-void put_fr(std::vector<uint8_t>& out, const Fr& x);
-void put_g1(std::vector<uint8_t>& out, const G1AffineH& p);
-void put_g2(std::vector<uint8_t>& out, const G2AffineH& p);
 // the Groth16 key and the public signals as the first challenge hashes them
 void put_vkey(std::vector<uint8_t>& out, const VerifyingKey& vk);
-// reads a canonical coordinate; throws if it is not below q
-Fq fq_at(const uint8_t* p);
-G1AffineH g1_at(const uint8_t* p);   // + on the curve
-G2AffineH g2_at(const uint8_t* p);   // + on the twist and in the order-r subgroup
+G1AffineH g1_at(const uint8_t* p);   // load_g1 + on the curve
+G2AffineH g2_at(const uint8_t* p);   // load_g2 + on the twist and in the order-r subgroup
 
 // Coefficients (low to high) of the folded-key polynomials after the rounds with challenges xs:
 //   v: f_v(X) = prod_j (1 + x_j^-1 (X / r)^(n / 2^(j+1))), n coefficients

@@ -104,6 +104,20 @@ G2AffineH g2_generator();
 bool g1_on_curve(const G1AffineH& p);
 bool g2_on_curve(const G2AffineH& p);
 
+// Host byte format (pairing_host.cpp): 32-byte little-endian standard form; G1 = x, y; G2 = x.c0, x.c1, y.c0, y.c1;
+// infinity = all zero.  put_* append to `out`.  The readers throw "<what> not reduced" on a coordinate not below q;
+// whether a point must be on its curve or in its subgroup is the caller's policy.
+void store_fq(uint8_t* out, const Fq& x);
+void store_fr(uint8_t* out, const Fr& x);
+void store_g1(uint8_t* out, const G1AffineH& p);
+void store_g2(uint8_t* out, const G2AffineH& p);
+void put_fr(std::vector<uint8_t>& out, const Fr& x);
+void put_g1(std::vector<uint8_t>& out, const G1AffineH& p);
+void put_g2(std::vector<uint8_t>& out, const G2AffineH& p);
+Fq fq_at(const uint8_t* p, const char* what = "coordinate");
+G1AffineH load_g1(const uint8_t* p, const char* what = "coordinate");
+G2AffineH load_g2(const uint8_t* p, const char* what = "coordinate");
+
 // Host mirror of the device accumulator (extended Jacobian, x = X/ZZ, y = Y/ZZZ); same memory image.
 template <class F>
 struct XyzzH {

@@ -847,8 +847,6 @@ static int do_check(zke_ctx* x, zke_ctx::Slot& S, size_t batch, int32_t* status,
     return bad;
 }
 
-static void write_fq(uint8_t* dst, const Fq& x) { U256 s = x.to_u256(); memcpy(dst, s.v, 32); }
-
 // Serial tail of one MSM on the host: sum of the unit-scalar partials + Horner over the window sums.
 template <class F>
 static AffineH<F> finish_msm(const uint8_t* block, const dev::MsmConfig& cfg) {
@@ -861,6 +859,51 @@ static AffineH<F> finish_msm(const uint8_t* block, const dev::MsmConfig& cfg) {
     }
     if (cfg.classify) for (int i = 0; i < dev::MSM_ONES_SLOTS; ++i) acc.add(slots[i]);
     return acc.to_affine();
+}
+
+// Enqueues the witness multi-exponentiations A, B1, C and B2 over the wires [lo, hi) on `st`, in that order, into their
+// blocks of `res`; `queued(stage)` runs after each one is queued.
+template <class Queued>
+static void enqueue_witness_msms(const zke_ctx* x, const uint8_t* w, uint32_t lo, uint32_t hi, uint8_t* ws, uint8_t* res,
+                                 cudaStream_t st, Queued queued) {
+    const zke_zkey* zk = x->zkey;
+    w += 32ull * lo;
+    dev::MsmPlan<dev::Fq>::run(zk->A.p + 64ull * lo, w, hi - lo, x->cfg_w, ws, res + RES_A * ZKE_RES_G1_BLOCK, st);
+    queued(ZKE_STAGE_MSM_A);
+    dev::MsmPlan<dev::Fq>::run(zk->B1.p + 64ull * lo, w, hi - lo, x->cfg_w, ws, res + RES_B1 * ZKE_RES_G1_BLOCK, st);
+    queued(ZKE_STAGE_MSM_B1);
+    dev::MsmPlan<dev::Fq>::run(zk->C.p + 64ull * lo, w, hi - lo, x->cfg_w, ws, res + RES_C * ZKE_RES_G1_BLOCK, st);
+    queued(ZKE_STAGE_MSM_C);
+    dev::MsmPlan<dev::Fq2>::run(zk->B2.p + 128ull * lo, w, hi - lo, x->cfg_w, ws, res + RES_B2 * ZKE_RES_G1_BLOCK, st);
+    CHECK_LAUNCH();
+    queued(ZKE_STAGE_MSM_B2);
+}
+
+struct MsmSums { G1AffineH a, b1, c, h; G2AffineH b2; };
+
+// The host tail of the five multi-exponentiations of a result buffer copied back from the device
+static MsmSums finish_msms(const uint8_t* res, const dev::MsmConfig& cfg_w, const dev::MsmConfig& cfg_h) {
+    return MsmSums{finish_msm<Fq>(res + RES_A * ZKE_RES_G1_BLOCK, cfg_w), finish_msm<Fq>(res + RES_B1 * ZKE_RES_G1_BLOCK, cfg_w),
+                   finish_msm<Fq>(res + RES_C * ZKE_RES_G1_BLOCK, cfg_w), finish_msm<Fq>(res + RES_H * ZKE_RES_G1_BLOCK, cfg_h),
+                   finish_msm<Fq2>(res + RES_B2 * ZKE_RES_G1_BLOCK, cfg_w)};
+}
+
+// The proving key's fixed points that the assembly of a proof adds
+struct KeyPoints { G1AffineH alpha1, beta1, delta1; G2AffineH beta2, delta2; };
+
+// Writes the 256-byte proof pi_A, pi_B, pi_C:  pi_A = alpha1 + A + r delta1 ; pi_B = beta2 + B2 + s delta2 ;
+// pi_C = C + H + s pi_A + r pi_B1 - r s delta1 with pi_B1 = beta1 + B1 + s delta1
+static void assemble_proof(const KeyPoints& kp, const G1JacH& a, const G1JacH& b1, const G1JacH& c, const G1JacH& h, const G2JacH& b2,
+                           const U256& r, const U256& s, uint8_t out[256]) {
+    const G1JacH delta1 = G1JacH::from_affine(kp.delta1);
+    const G1JacH pa = G1JacH::from_affine(kp.alpha1).add(a).add(delta1.mul(r));
+    const G2JacH pb2 = G2JacH::from_affine(kp.beta2).add(b2).add(G2JacH::from_affine(kp.delta2).mul(s));
+    const G1JacH pb1 = G1JacH::from_affine(kp.beta1).add(b1).add(delta1.mul(s));
+    const U256 rs_prod = (Fr::from_u256(r) * Fr::from_u256(s)).to_u256();
+    const G1JacH pc = c.add(h).add(pa.mul(s)).add(pb1.mul(r)).add(delta1.mul(rs_prod).neg());
+    store_g1(out, pa.to_affine());
+    store_g2(out + 64, pb2.to_affine());
+    store_g1(out + 192, pc.to_affine());
 }
 
 static void sync_lanes(zke_ctx* x) {
@@ -901,10 +944,11 @@ static void enqueue_prove(zke_ctx* x, zke_ctx::Slot& S, size_t batch, const uint
         size_t t0 = 0, t1 = 0;
         CUDA_OK(cudaMemsetAsync(flag, 0xff, 4, st));
         if (prof) t0 = x->mark(st);
+        auto span = [&](int stage) { if (prof) { t1 = x->mark(st); x->spans.push_back({stage, t0, t1}); t0 = t1; } };
         // `hv` = the lane's low-priority stream for the saturating kernels (profiling: everything on `st`)
         cudaStream_t hv = (prof || !x->split_streams) ? st : L.heavy;
         dev::launch_build_ab(x->r1cs, w, L.va.p, L.vb.p, L.vc.p, N, flag, st);
-        if (prof) { t1 = x->mark(st); x->spans.push_back({ZKE_STAGE_MATVEC, t0, t1}); t0 = t1; }
+        span(ZKE_STAGE_MATVEC);
         if (hv != st) { CUDA_OK(cudaEventRecord(L.ev[0], st)); CUDA_OK(cudaStreamWaitEvent(hv, L.ev[0], 0)); }
         dev::launch_intt_dif(L.va.p, x->ntt, x->coset_scale.p, hv);
         dev::launch_intt_dif(L.vb.p, x->ntt, x->coset_scale.p, hv);
@@ -915,33 +959,17 @@ static void enqueue_prove(zke_ctx* x, zke_ctx::Slot& S, size_t batch, const uint
         dev::launch_quotient(L.va.p, L.vb.p, L.vc.p, L.vd.p, N, hv);
         CHECK_LAUNCH();
         if (hv != st) CUDA_OK(cudaEventRecord(L.ev[1], hv));
-        if (prof) { t1 = x->mark(st); x->spans.push_back({ZKE_STAGE_NTT, t0, t1}); t0 = t1; }
+        span(ZKE_STAGE_NTT);
         // the witness MSMs do not depend on the transforms: with split streams they run on `st` while the lane's NTT
         // passes are still in flight on `hv` (the MSM workspace is only touched from `st`-ordered work)
-        uint8_t* ws_w = L.msm_ws.p;
-        dev::MsmPlan<dev::Fq>::run(zk->A.p, w, m, x->cfg_w, ws_w, res + 0 * ZKE_RES_G1_BLOCK, st);
-        if (prof) { t1 = x->mark(st); x->spans.push_back({ZKE_STAGE_MSM_A, t0, t1}); t0 = t1; }
-        dev::MsmPlan<dev::Fq>::run(zk->B1.p, w, m, x->cfg_w, ws_w, res + 1 * ZKE_RES_G1_BLOCK, st);
-        if (prof) { t1 = x->mark(st); x->spans.push_back({ZKE_STAGE_MSM_B1, t0, t1}); t0 = t1; }
-        dev::MsmPlan<dev::Fq>::run(zk->C.p, w, m, x->cfg_w, ws_w, res + 2 * ZKE_RES_G1_BLOCK, st);
-        if (prof) { t1 = x->mark(st); x->spans.push_back({ZKE_STAGE_MSM_C, t0, t1}); t0 = t1; }
-        dev::MsmPlan<dev::Fq2>::run(zk->B2.p, w, m, x->cfg_w, ws_w, res + 4 * ZKE_RES_G1_BLOCK, st);
-        CHECK_LAUNCH();
-        if (prof) { t1 = x->mark(st); x->spans.push_back({ZKE_STAGE_MSM_B2, t0, t1}); t0 = t1; }
+        enqueue_witness_msms(x, w, 0, m, L.msm_ws.p, res, st, span);
         if (hv != st) CUDA_OK(cudaStreamWaitEvent(st, L.ev[1], 0));
-        {
-            dev::MsmPlan<dev::Fq>::Heavy heavy{hv, L.ev[2], L.ev[3]};
-            if (prof) {
-                size_t i0, i1;
-                cudaEvent_t evs[2];
-                evs[0] = x->ev(&i0); evs[1] = x->ev(&i1);
-                dev::MsmPlan<dev::Fq>::run(zk->H.p, L.vd.p, N, x->cfg_h, L.msm_ws.p, res + 3 * ZKE_RES_G1_BLOCK, st, evs, &heavy);
-                x->spans.push_back({ZKE_STAGE_MSM_H_BUCKETS, i0, i1});
-                t1 = x->mark(st); x->spans.push_back({ZKE_STAGE_MSM_H, t0, t1}); t0 = t1;
-            } else {
-                dev::MsmPlan<dev::Fq>::run(zk->H.p, L.vd.p, N, x->cfg_h, L.msm_ws.p, res + 3 * ZKE_RES_G1_BLOCK, st, nullptr, &heavy);
-            }
-        }
+        const dev::MsmPlan<dev::Fq>::Heavy heavy{hv, L.ev[2], L.ev[3]};
+        size_t i0 = 0, i1 = 0;
+        cudaEvent_t evs[2] = {prof ? x->ev(&i0) : nullptr, prof ? x->ev(&i1) : nullptr};   // profiling: the bucket kernel alone
+        dev::MsmPlan<dev::Fq>::run(zk->H.p, L.vd.p, N, x->cfg_h, L.msm_ws.p, res + RES_H * ZKE_RES_G1_BLOCK, st, prof ? evs : nullptr, &heavy);
+        if (prof) x->spans.push_back({ZKE_STAGE_MSM_H_BUCKETS, i0, i1});
+        span(ZKE_STAGE_MSM_H);
         CHECK_LAUNCH();
         CUDA_OK(cudaMemcpyAsync(S.results_host + (size_t)ZKE_RESULT_STRIDE * e, res, ZKE_RESULT_STRIDE, cudaMemcpyDeviceToHost, st));
         CUDA_OK(cudaEventRecord(S.done[e], st));
@@ -958,8 +986,7 @@ static int finish_prove(zke_ctx* x, zke_ctx::Slot& S, uint8_t* proofs_out, uint8
     const zke_zkey* zk = x->zkey;
     const size_t batch = S.batch;
     const uint32_t l = x->n_public;
-    const G1JacH alpha1 = G1JacH::from_affine(zk->alpha1), beta1 = G1JacH::from_affine(zk->beta1), delta1 = G1JacH::from_affine(zk->delta1);
-    const G2JacH beta2 = G2JacH::from_affine(zk->beta2), delta2 = G2JacH::from_affine(zk->delta2);
+    const KeyPoints kp{zk->alpha1, zk->beta1, zk->delta1, zk->beta2, zk->delta2};
     std::vector<int32_t> st_local(batch, -1);
     std::string first_error;
     std::mutex err_mutex;
@@ -975,22 +1002,9 @@ static int finish_prove(zke_ctx* x, zke_ctx::Slot& S, uint8_t* proofs_out, uint8
         U256 r, sc;
         if (!S.rs.empty()) { memcpy(r.v, S.rs.data() + 64 * e, 32); memcpy(sc.v, S.rs.data() + 64 * e + 32, 32); }
         else { random_scalar(r); random_scalar(sc); }
-        G1AffineH ma = finish_msm<Fq>(res + 0 * ZKE_RES_G1_BLOCK, x->cfg_w);
-        G1AffineH mb1 = finish_msm<Fq>(res + 1 * ZKE_RES_G1_BLOCK, x->cfg_w);
-        G1AffineH mc = finish_msm<Fq>(res + 2 * ZKE_RES_G1_BLOCK, x->cfg_w);
-        G1AffineH mh = finish_msm<Fq>(res + 3 * ZKE_RES_G1_BLOCK, x->cfg_h);
-        G2AffineH mb2 = finish_msm<Fq2>(res + 4 * ZKE_RES_G1_BLOCK, x->cfg_w);
-        // pi_A = alpha + A + r delta ; pi_B = beta + B + s delta ; pi_C = C + H + s pi_A + r pi_B1 - r s delta
-        G1JacH pa = alpha1.add(G1JacH::from_affine(ma)).add(delta1.mul(r));
-        G2JacH pb2 = beta2.add(G2JacH::from_affine(mb2)).add(delta2.mul(sc));
-        G1JacH pb1 = beta1.add(G1JacH::from_affine(mb1)).add(delta1.mul(sc));
-        U256 rs_prod = (Fr::from_u256(r) * Fr::from_u256(sc)).to_u256();
-        G1JacH pc = G1JacH::from_affine(mc).add(G1JacH::from_affine(mh)).add(pa.mul(sc)).add(pb1.mul(r)).add(delta1.mul(rs_prod).neg());
-        G1AffineH A = pa.to_affine(), C = pc.to_affine();
-        G2AffineH B = pb2.to_affine();
-        write_fq(out + 0, A.x); write_fq(out + 32, A.y);
-        write_fq(out + 64, B.x.c0); write_fq(out + 96, B.x.c1); write_fq(out + 128, B.y.c0); write_fq(out + 160, B.y.c1);
-        write_fq(out + 192, C.x); write_fq(out + 224, C.y);
+        const MsmSums m = finish_msms(res, x->cfg_w, x->cfg_h);
+        assemble_proof(kp, G1JacH::from_affine(m.a), G1JacH::from_affine(m.b1), G1JacH::from_affine(m.c), G1JacH::from_affine(m.h),
+                       G2JacH::from_affine(m.b2), r, sc, out);
     };
     const int T = (int)std::max<size_t>(1, std::min<size_t>((size_t)x->finish_threads, batch));
     std::atomic<size_t> next{0};
@@ -1144,7 +1158,20 @@ static void shard_mid(zke_ctx* x) {
     x->shard_stage = 2;
 }
 
-static void put_g1(uint8_t* dst, const G1AffineH& p) { write_fq(dst, p.x); write_fq(dst + 32, p.y); }
+// A GPU's share of a proof (ZKE_SHARD_PARTIAL_BYTES): A, B1, C, H, B2 in the host point format, then the first violated
+// row of its rows (u32).  The reader refuses unreduced coordinates and points off their curves (no subgroup check).
+static const char PARTIAL_COORD[] = "partial point coordinate";
+static void write_partial(const MsmSums& m, uint32_t first_bad, uint8_t* out) {
+    store_g1(out, m.a); store_g1(out + 64, m.b1); store_g1(out + 128, m.c); store_g1(out + 192, m.h); store_g2(out + 256, m.b2);
+    memcpy(out + 384, &first_bad, 4);
+}
+static MsmSums read_partial(const uint8_t* p, uint32_t& first_bad) {
+    const MsmSums m{load_g1(p, PARTIAL_COORD), load_g1(p + 64, PARTIAL_COORD), load_g1(p + 128, PARTIAL_COORD),
+                    load_g1(p + 192, PARTIAL_COORD), load_g2(p + 256, PARTIAL_COORD)};
+    if (!g1_on_curve(m.a) || !g1_on_curve(m.b1) || !g1_on_curve(m.c) || !g1_on_curve(m.h) || !g2_on_curve(m.b2)) throw std::runtime_error("partial point not on the curve");
+    memcpy(&first_bad, p + 384, 4);
+    return m;
+}
 
 static void shard_end(zke_ctx* x, uint8_t* partial_out, uint8_t* publics_out) {
     if (x->shard_stage != 2) throw std::runtime_error("zke_shard_end out of order");
@@ -1166,51 +1193,29 @@ static void shard_end(zke_ctx* x, uint8_t* partial_out, uint8_t* publics_out) {
     CHECK_LAUNCH();
     // witness multi-exponentiations over this GPU's point range, H over its columns (all other scalars are zero)
     const uint32_t lo = (uint32_t)((uint64_t)m * x->shard_rank / G), hi = (uint32_t)((uint64_t)m * (x->shard_rank + 1) / G);
-    const uint8_t* w = S.w_all.p;
     uint8_t* res = S.results.p;
-    dev::MsmPlan<dev::Fq>::run(zk->A.p + 64ull * lo, w + 32ull * lo, hi - lo, x->cfg_w, L.msm_ws.p, res + 0 * ZKE_RES_G1_BLOCK, st);
-    dev::MsmPlan<dev::Fq>::run(zk->B1.p + 64ull * lo, w + 32ull * lo, hi - lo, x->cfg_w, L.msm_ws.p, res + 1 * ZKE_RES_G1_BLOCK, st);
-    dev::MsmPlan<dev::Fq>::run(zk->C.p + 64ull * lo, w + 32ull * lo, hi - lo, x->cfg_w, L.msm_ws.p, res + 2 * ZKE_RES_G1_BLOCK, st);
-    dev::MsmPlan<dev::Fq2>::run(zk->B2.p + 128ull * lo, w + 32ull * lo, hi - lo, x->cfg_w, L.msm_ws.p, res + 4 * ZKE_RES_G1_BLOCK, st);
-    dev::MsmPlan<dev::Fq>::run(zk->H.p, L.vd.p, N, x->cfg_h, L.msm_ws.p, res + 3 * ZKE_RES_G1_BLOCK, st);
+    enqueue_witness_msms(x, S.w_all.p, lo, hi, L.msm_ws.p, res, st, [](int) {});
+    dev::MsmPlan<dev::Fq>::run(zk->H.p, L.vd.p, N, x->cfg_h, L.msm_ws.p, res + RES_H * ZKE_RES_G1_BLOCK, st);
     CHECK_LAUNCH();
     CUDA_OK(cudaMemcpyAsync(S.results_host, res, ZKE_RESULT_STRIDE, cudaMemcpyDeviceToHost, st));
     if (l) CUDA_OK(cudaMemcpyAsync(S.publics_host, S.w_all.p + 32, (size_t)l * 32, cudaMemcpyDeviceToHost, st));
     CUDA_OK(cudaStreamSynchronize(st));
-    const uint8_t* rh = S.results_host;
-    put_g1(partial_out + 0, finish_msm<Fq>(rh + 0 * ZKE_RES_G1_BLOCK, x->cfg_w));
-    put_g1(partial_out + 64, finish_msm<Fq>(rh + 1 * ZKE_RES_G1_BLOCK, x->cfg_w));
-    put_g1(partial_out + 128, finish_msm<Fq>(rh + 2 * ZKE_RES_G1_BLOCK, x->cfg_w));
-    put_g1(partial_out + 192, finish_msm<Fq>(rh + 3 * ZKE_RES_G1_BLOCK, x->cfg_h));
-    const G2AffineH b2 = finish_msm<Fq2>(rh + 4 * ZKE_RES_G1_BLOCK, x->cfg_w);
-    write_fq(partial_out + 256, b2.x.c0); write_fq(partial_out + 288, b2.x.c1); write_fq(partial_out + 320, b2.y.c0); write_fq(partial_out + 352, b2.y.c1);
-    memcpy(partial_out + 384, rh + ZKE_RES_FLAG_OFF, 4);     // first violated row among this GPU's rows (0xffffffff: none)
+    uint32_t first_bad;     // first violated row among this GPU's rows (0xffffffff: none)
+    memcpy(&first_bad, S.results_host + ZKE_RES_FLAG_OFF, 4);
+    write_partial(finish_msms(S.results_host, x->cfg_w, x->cfg_h), first_bad, partial_out);
     if (publics_out && l) memcpy(publics_out, S.publics_host, (size_t)l * 32);
     x->shard_stage = 0;
 }
 
-static Fq fq_from_le(const uint8_t* b) {
-    U256 v;
-    memcpy(v.v, b, 32);
-    if (u256_cmp(v, fq_params().p) >= 0) throw std::runtime_error("partial point coordinate not reduced");
-    return Fq::from_u256(v);
-}
-
-// host only: sums the partial points of all GPUs and assembles the proof (same formulas as finish_prove)
-struct ShardKeyPoints { G1AffineH alpha1, beta1, delta1; G2AffineH beta2, delta2; };
-static int shard_combine(const ShardKeyPoints* zk, const uint8_t* partials, int world, const uint8_t* rs, uint8_t* out, int32_t* status) {
+// host only: sums the partial points of all GPUs and assembles the proof
+static int shard_combine(const KeyPoints& kp, const uint8_t* partials, int world, const uint8_t* rs, uint8_t* out, int32_t* status) {
     G1JacH sa = G1JacH::inf(), sb1 = G1JacH::inf(), sc = G1JacH::inf(), sh = G1JacH::inf();
     G2JacH sb2 = G2JacH::inf();
     uint32_t first_bad = 0xffffffffu;
     for (int r = 0; r < world; ++r) {
-        const uint8_t* p = partials + (size_t)ZKE_SHARD_PARTIAL_BYTES * r;
-        auto g1 = [&](const uint8_t* q) { return G1AffineH{fq_from_le(q), fq_from_le(q + 32)}; };
-        const G1AffineH a = g1(p), b1 = g1(p + 64), c = g1(p + 128), h = g1(p + 192);
-        const G2AffineH b2{Fq2{fq_from_le(p + 256), fq_from_le(p + 288)}, Fq2{fq_from_le(p + 320), fq_from_le(p + 352)}};
-        if (!g1_on_curve(a) || !g1_on_curve(b1) || !g1_on_curve(c) || !g1_on_curve(h) || !g2_on_curve(b2)) throw std::runtime_error("partial point not on the curve");
-        sa = sa.add_affine(a); sb1 = sb1.add_affine(b1); sc = sc.add_affine(c); sh = sh.add_affine(h); sb2 = sb2.add_affine(b2);
         uint32_t f;
-        memcpy(&f, p + 384, 4);
+        const MsmSums m = read_partial(partials + (size_t)ZKE_SHARD_PARTIAL_BYTES * r, f);
+        sa = sa.add_affine(m.a); sb1 = sb1.add_affine(m.b1); sc = sc.add_affine(m.c); sh = sh.add_affine(m.h); sb2 = sb2.add_affine(m.b2);
         first_bad = std::min(first_bad, f);
     }
     if (status) *status = first_bad == 0xffffffffu ? -1 : (int32_t)first_bad;
@@ -1219,18 +1224,7 @@ static int shard_combine(const ShardKeyPoints* zk, const uint8_t* partials, int 
     if (rs) { memcpy(r.v, rs, 32); memcpy(s.v, rs + 32, 32); }
     else { random_scalar(r); random_scalar(s); }
     if (u256_cmp(r, fr_params().p) >= 0 || u256_cmp(s, fr_params().p) >= 0) throw std::runtime_error("r / s not reduced mod the group order");
-    const G1JacH alpha1 = G1JacH::from_affine(zk->alpha1), beta1 = G1JacH::from_affine(zk->beta1), delta1 = G1JacH::from_affine(zk->delta1);
-    const G2JacH beta2 = G2JacH::from_affine(zk->beta2), delta2 = G2JacH::from_affine(zk->delta2);
-    G1JacH pa = alpha1.add(sa).add(delta1.mul(r));
-    G2JacH pb2 = beta2.add(sb2).add(delta2.mul(s));
-    G1JacH pb1 = beta1.add(sb1).add(delta1.mul(s));
-    U256 rs_prod = (Fr::from_u256(r) * Fr::from_u256(s)).to_u256();
-    G1JacH pc = sc.add(sh).add(pa.mul(s)).add(pb1.mul(r)).add(delta1.mul(rs_prod).neg());
-    G1AffineH A = pa.to_affine(), C = pc.to_affine();
-    G2AffineH B = pb2.to_affine();
-    write_fq(out + 0, A.x); write_fq(out + 32, A.y);
-    write_fq(out + 64, B.x.c0); write_fq(out + 96, B.x.c1); write_fq(out + 128, B.y.c0); write_fq(out + 160, B.y.c1);
-    write_fq(out + 192, C.x); write_fq(out + 224, C.y);
+    assemble_proof(kp, sa, sb1, sc, sh, sb2, r, s, out);
     return 0;
 }
 
@@ -1287,7 +1281,7 @@ int64_t zke_zkey_section(const zke_zkey* z, int section, uint8_t* out, size_t ca
         auto g1_host = [&](const G1AffineH* pts, size_t n) -> int64_t {
             if (!out) return (int64_t)n;
             if (cap < n * 64) return -2;
-            for (size_t i = 0; i < n; ++i) { write_fq(out + 64 * i, pts[i].x); write_fq(out + 64 * i + 32, pts[i].y); }
+            for (size_t i = 0; i < n; ++i) store_g1(out + 64 * i, pts[i]);
             return (int64_t)n;
         };
         auto g1_dev = [&](const DevBuf& b, size_t n) -> int64_t {
@@ -1299,10 +1293,7 @@ int64_t zke_zkey_section(const zke_zkey* z, int section, uint8_t* out, size_t ca
         auto g2_host = [&](const G2AffineH* pts, size_t n) -> int64_t {
             if (!out) return (int64_t)n;
             if (cap < n * 128) return -2;
-            for (size_t i = 0; i < n; ++i) {
-                write_fq(out + 128 * i, pts[i].x.c0); write_fq(out + 128 * i + 32, pts[i].x.c1);
-                write_fq(out + 128 * i + 64, pts[i].y.c0); write_fq(out + 128 * i + 96, pts[i].y.c1);
-            }
+            for (size_t i = 0; i < n; ++i) store_g2(out + 128 * i, pts[i]);
             return (int64_t)n;
         };
         switch (section) {
@@ -1520,8 +1511,8 @@ int zke_shard_combine(const zke_zkey* z, const uint8_t* partials, int world, con
                       char* err, size_t errcap) {
     try {
         if (!z || !partials || !proof_out || world < 1) throw std::runtime_error("bad argument");
-        const ShardKeyPoints kp{z->alpha1, z->beta1, z->delta1, z->beta2, z->delta2};
-        int bad = shard_combine(&kp, partials, world, rs, proof_out, status);
+        const KeyPoints kp{z->alpha1, z->beta1, z->delta1, z->beta2, z->delta2};
+        int bad = shard_combine(kp, partials, world, rs, proof_out, status);
         if (bad) set_err(err, errcap, "Assert Failed: constraint " + std::to_string(status ? *status : 0));
         return bad;
     } catch (const std::exception& e) { set_err(err, errcap, e.what()); return -1; }
@@ -1530,10 +1521,9 @@ int zke_shard_combine_raw(const uint8_t* key_points, const uint8_t* partials, in
                           int32_t* status, char* err, size_t errcap) {
     try {
         if (!key_points || !partials || !proof_out || world < 1) throw std::runtime_error("bad argument");
-        auto g1 = [&](const uint8_t* q) { return G1AffineH{fq_from_le(q), fq_from_le(q + 32)}; };
-        auto g2 = [&](const uint8_t* q) { return G2AffineH{Fq2{fq_from_le(q), fq_from_le(q + 32)}, Fq2{fq_from_le(q + 64), fq_from_le(q + 96)}}; };
-        const ShardKeyPoints kp{g1(key_points), g1(key_points + 64), g1(key_points + 128), g2(key_points + 192), g2(key_points + 320)};
-        int bad = shard_combine(&kp, partials, world, rs, proof_out, status);
+        const KeyPoints kp{load_g1(key_points, PARTIAL_COORD), load_g1(key_points + 64, PARTIAL_COORD), load_g1(key_points + 128, PARTIAL_COORD),
+                          load_g2(key_points + 192, PARTIAL_COORD), load_g2(key_points + 320, PARTIAL_COORD)};
+        int bad = shard_combine(kp, partials, world, rs, proof_out, status);
         if (bad) set_err(err, errcap, "Assert Failed: constraint " + std::to_string(status ? *status : 0));
         return bad;
     } catch (const std::exception& e) { set_err(err, errcap, e.what()); return -1; }

@@ -18,6 +18,7 @@ struct zke_circuit {
 
 // per-email result block: the MSM result blocks (msm.cuh: 64 XYZZ slots each) of A, B1, C, H (G1, 128-byte slots)
 // followed by B2 (G2, 256-byte slots), then the first-violated-constraint word
+enum ZkeResBlock { RES_A = 0, RES_B1 = 1, RES_C = 2, RES_H = 3, RES_B2 = 4 };   // block b at b * ZKE_RES_G1_BLOCK
 #define ZKE_RES_G1_BLOCK (64 * 128)
 #define ZKE_RES_G2_BLOCK (64 * 256)
 #define ZKE_RES_FLAG_OFF (4 * ZKE_RES_G1_BLOCK + ZKE_RES_G2_BLOCK)

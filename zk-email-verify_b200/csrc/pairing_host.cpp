@@ -33,6 +33,25 @@ bool g2_on_curve(const G2AffineH& p) {
     return p.y.sqr() == p.x.sqr() * p.x + twist_b();
 }
 
+void store_fq(uint8_t* out, const Fq& x) { const U256 s = x.to_u256(); memcpy(out, s.v, 32); }
+void store_fr(uint8_t* out, const Fr& x) { const U256 s = x.to_u256(); memcpy(out, s.v, 32); }
+void store_g1(uint8_t* out, const G1AffineH& p) { store_fq(out, p.x); store_fq(out + 32, p.y); }
+void store_g2(uint8_t* out, const G2AffineH& p) { store_fq(out, p.x.c0); store_fq(out + 32, p.x.c1); store_fq(out + 64, p.y.c0); store_fq(out + 96, p.y.c1); }
+void put_fr(std::vector<uint8_t>& out, const Fr& x) { out.resize(out.size() + 32); store_fr(&out[out.size() - 32], x); }
+void put_g1(std::vector<uint8_t>& out, const G1AffineH& p) { out.resize(out.size() + 64); store_g1(&out[out.size() - 64], p); }
+void put_g2(std::vector<uint8_t>& out, const G2AffineH& p) { out.resize(out.size() + 128); store_g2(&out[out.size() - 128], p); }
+
+Fq fq_at(const uint8_t* p, const char* what) {
+    U256 x;
+    memcpy(x.v, p, 32);
+    if (u256_cmp(x, fq_params().p) >= 0) throw std::runtime_error(std::string(what) + " not reduced");
+    return Fq::from_u256(x);
+}
+G1AffineH load_g1(const uint8_t* p, const char* what) { return G1AffineH{fq_at(p, what), fq_at(p + 32, what)}; }
+G2AffineH load_g2(const uint8_t* p, const char* what) {
+    return G2AffineH{Fq2{fq_at(p, what), fq_at(p + 32, what)}, Fq2{fq_at(p + 64, what), fq_at(p + 96, what)}};
+}
+
 namespace {
 
 struct F12 {
@@ -222,9 +241,8 @@ void gt_store(const Gt& e, uint8_t out[384]) {
     for (int i = 0; i < 2; ++i)
         for (int j = 0; j < 3; ++j) {
             const int n = 2 * j + i;
-            const U256 a = (e.c[n] + nine * e.c[n + 6]).to_u256(), b = e.c[n + 6].to_u256();
-            memcpy(out + 64 * (3 * i + j), a.v, 32);
-            memcpy(out + 64 * (3 * i + j) + 32, b.v, 32);
+            store_fq(out + 64 * (3 * i + j), e.c[n] + nine * e.c[n + 6]);
+            store_fq(out + 64 * (3 * i + j) + 32, e.c[n + 6]);
         }
 }
 Gt gt_load(const uint8_t* in) {

@@ -230,9 +230,10 @@ namespace {
 
 unsigned blocks(size_t threads) { return (unsigned)((threads + dev::VERIFY_THREADS - 1) / dev::VERIFY_THREADS); }
 
-void put_fq(std::vector<uint8_t>& out, const Fq& x) { const uint8_t* b = reinterpret_cast<const uint8_t*>(x.m.v); out.insert(out.end(), b, b + 32); }
-void put_g1(std::vector<uint8_t>& out, const G1AffineH& p) { put_fq(out, p.x); put_fq(out, p.y); }
-void put_g2(std::vector<uint8_t>& out, const G2AffineH& p) { put_fq(out, p.x.c0); put_fq(out, p.x.c1); put_fq(out, p.y.c0); put_fq(out, p.y.c1); }
+// Montgomery images of points, the format the verification kernels read (not the standard form of ec_host.hpp)
+void put_fq_mont(std::vector<uint8_t>& out, const Fq& x) { const uint8_t* b = reinterpret_cast<const uint8_t*>(x.m.v); out.insert(out.end(), b, b + 32); }
+void put_g1_mont(std::vector<uint8_t>& out, const G1AffineH& p) { put_fq_mont(out, p.x); put_fq_mont(out, p.y); }
+void put_g2_mont(std::vector<uint8_t>& out, const G2AffineH& p) { put_fq_mont(out, p.x.c0); put_fq_mont(out, p.x.c1); put_fq_mont(out, p.y.c0); put_fq_mont(out, p.y.c1); }
 
 // Folds `count` rows of `width` elements to one row, level by level between two scratch buffers; returns the row
 template <class Op>
@@ -289,9 +290,9 @@ zke_verifier* zke_verifier_open(const char* vkey_json, int device, char* err, si
         select_device(device);
         CUDA_OK(cudaStreamCreateWithFlags(&v->stream, cudaStreamNonBlocking));
         std::vector<uint8_t> ic, alpha, g2;
-        for (auto& p : vk.ic) put_g1(ic, p);
-        put_g1(alpha, vk.alpha1);
-        for (int k = 0; k < 3; ++k) put_g2(g2, *g2s[k]);
+        for (auto& p : vk.ic) put_g1_mont(ic, p);
+        put_g1_mont(alpha, vk.alpha1);
+        for (int k = 0; k < 3; ++k) put_g2_mont(g2, *g2s[k]);
         CUDA_OK(cudaMemcpy(v->ic.reserve(ic.size()), ic.data(), ic.size(), cudaMemcpyHostToDevice));
         CUDA_OK(cudaMemcpy(v->alpha.reserve(64), alpha.data(), 64, cudaMemcpyHostToDevice));
         CUDA_OK(cudaMemcpy(v->g2.reserve(384), g2.data(), 384, cudaMemcpyHostToDevice));
@@ -406,14 +407,9 @@ int zke_selftest_pairing_gpu(int device, size_t n, const uint8_t* g1, const uint
     try {
         if (n == 0) return 0;
         if (!g1 || !g2 || !out) throw std::runtime_error("null argument");
-        auto fq_at = [](const uint8_t* b) {
-            U256 x; memcpy(x.v, b, 32);
-            if (u256_cmp(x, fq_params().p) >= 0) throw std::runtime_error("coordinate not reduced");
-            return Fq::from_u256(x);
-        };
         for (size_t i = 0; i < n; ++i) {
-            const G1AffineH p{fq_at(g1 + 64 * i), fq_at(g1 + 64 * i + 32)};
-            const G2AffineH q{Fq2{fq_at(g2 + 128 * i), fq_at(g2 + 128 * i + 32)}, Fq2{fq_at(g2 + 128 * i + 64), fq_at(g2 + 128 * i + 96)}};
+            const G1AffineH p = load_g1(g1 + 64 * i);
+            const G2AffineH q = load_g2(g2 + 128 * i);
             if (!g1_on_curve(p) || !g2_on_curve(q)) throw std::runtime_error("point " + std::to_string(i) + " is not on its curve");
         }
         select_device(device);
