@@ -322,6 +322,78 @@ def test_wide_seed_record_matches_oracle(case, monkeypatch):
     assert carried >= 12 and upper_reads >= 12
 
 
+CHUNK = 896                  # witness.cu: RX_CHUNK, positions per pass of the 64-state and compact seeding
+LONG_REGEX = [("<", False), ("abcdefghijklmnopqrstuvwxyz0123456789ABCDEFGH", True), (">", False)]
+LONG_LEN = 2000              # crosses the chunk boundaries at positions 896 and 1792
+NON_BYTE = 256 + 7
+
+
+def long_regex_messages(count: int = 3, seed: int = 11):
+    """`count` messages of LONG_LEN bytes plus one that fails.  At every chunk boundary a match of LONG_REGEX is 32 to 43
+    bytes into its literal (deep DFA states live in the carried set), with bytes >= 0x80 just before it and just after
+    it; in the last message the match at the second boundary breaks on a byte >= 0x80 right after the boundary.  The
+    extra message is the first one with a non-byte value just past the first boundary."""
+    lit = LONG_REGEX[1][0].encode()
+    rng = random.Random(seed)
+    alphabet = b"<>abcxyz019ABCD \r\n"
+    out = []
+    for k in range(count):
+        s = bytearray(rng.choice(alphabet) for _ in range(LONG_LEN))
+        for q, b in enumerate(range(CHUNK, LONG_LEN, CHUNK)):
+            depth = 32 + (5 * k + 3 * q) % (len(lit) - 32)       # literal bytes read by the end of the chunk
+            start = b - depth - 1                                  # the '<'
+            s[start - 2:start] = "é".encode()
+            s[start:start + 2 + len(lit)] = b"<" + lit + b">"
+            s[start + 2 + len(lit):start + 5 + len(lit)] = "日".encode()
+            if k == count - 1 and q == 1:
+                s[b] = 0xe9
+        out.append(list(s))
+    bad = list(out[0])
+    bad[CHUNK] = NON_BYTE
+    return out + [bad]
+
+
+def _carried_states(seed, msg):
+    """Per message byte, what the seeding carries to the next byte: the live-state mask (64-state shape) or the one live
+    state (compact shape)."""
+    if seed["mode"] == 0:
+        return live_sets(seed, msg)
+    q, out = seed["first"], []
+    for c in msg:
+        d = seed["table"][256 * q + min(c, 255)]
+        q = 0 if d == 0xff else d
+        out.append(q)
+    return out
+
+
+@pytest.mark.parametrize("style", [0, 1], ids=["zkregex", "compact"])
+def test_long_regex_messages_cross_chunk_boundaries(style, monkeypatch):
+    """The seeded signals of the messages tests/test_gpu_witness_edges.py runs hold the values a Python run of the recorded
+    table gives, and at both chunk boundaries those messages carry a state >= 32 (the high half of the 64-bit mask, or a
+    compact state number >= 32) into the next chunk, with bytes >= 0x80 within 16 bytes of the boundary."""
+    from test_regex_seed_table import _check, _seeds
+    monkeypatch.setenv("ZKE_REGEX_STYLE", str(style))
+    c = z.Circuit.from_regex(LONG_REGEX, LONG_LEN)
+    seeds = _seeds(c)
+    assert len(seeds) == 1 and seeds[0]["mode"] == style and 32 < seeds[0]["n_states"] <= 64
+    msgs = long_regex_messages()
+    for msg in msgs[:-1]:
+        assert _check(c, {"msg": msg}, [msg]) > LONG_LEN
+        carried = _carried_states(seeds[0], msg)
+        for b in range(CHUNK, LONG_LEN, CHUNK):
+            assert (carried[b - 1] >> 32 if style == 0 else carried[b - 1] >= 32), (b, carried[b - 1])
+            assert any(x >= 0x80 for x in msg[b - 16:b + 16])
+    # a non-byte value fires no transition, as the marker 255 does; the zk-regex shape does not range-check its message,
+    # the compact shape does
+    bad = msgs[-1]
+    assert bad[CHUNK] == NON_BYTE and bad[:CHUNK] == msgs[0][:CHUNK]
+    if style == 0:
+        assert _check(c, {"msg": bad}, [bad]) > LONG_LEN
+    else:
+        with pytest.raises(AssertFailed, match="Num2Bits"):
+            oracle_witness(c, {"msg": bad})
+
+
 def test_more_than_255_states_stay_unseeded(monkeypatch):
     monkeypatch.setenv("ZKE_REGEX_STYLE", "0")
     c = z.Circuit.from_regex([("x", False), ("[a-z]" * 300, True)], 320)

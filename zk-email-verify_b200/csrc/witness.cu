@@ -283,7 +283,8 @@ __device__ void regex_coop(const DevProgram& P, uint8_t* w, uint32_t aux_off, un
 // in shared memory - computed once per email by the sequential division - and every call becomes three cooperative
 // products (column sums by 146 threads + one carry sweep): X = A B, q2 = floor(X / b^(t-1)) mu, q3 P, followed by at
 // most two corrective subtractions (Handbook of Applied Cryptography 14.42).  Falls back to the sequential routine when
-// the operands do not satisfy Barrett's preconditions (A, B >= b^t, or a modulus of fewer than four words).
+// the operands do not satisfy Barrett's preconditions (A, B >= b^t, a modulus of fewer than four words, or P = b^(t-1),
+// whose reciprocal does not fit t + 1 words).  tests/test_bigdiv_hint.py mirrors these decisions on the CPU.
 struct FpmulShared {
     uint32_t A[BIGDIV_MAXW], B[BIGDIV_MAXW], P[BIGDIV_MAXW + 1];
     uint32_t Pc[BIGDIV_MAXW + 1], mu[BIGDIV_MAXW + 2];     // cached modulus and its reciprocal
@@ -340,25 +341,26 @@ __device__ void fpmul_coop(const DevProgram& P, uint8_t* w, uint32_t aux_off, ui
         S.t = t;
         bool fits = t >= 4;
         for (int i = t; i < W && fits; ++i) fits = S.A[i] == 0 && S.B[i] == 0;       // A, B < b^t  =>  A B < b^(2t)
+        // P = b^(t-1) exactly: the reciprocal b^(t+1) needs t + 2 words, and bd_knuth_div writes only t + 1 quotient
+        // words (it would leave b^(t+1) - 1) - sequential path
+        bool power = fits && S.P[t - 1] == 1;
+        for (int i = 0; i < t - 1 && power; ++i) power = S.P[i] == 0;
+        if (power) fits = false;
         S.mode = fits ? 1 : 0;
         if (fits) {
             bool same = S.t_cached == t;
             for (int i = 0; i < t && same; ++i) same = S.Pc[i] == S.P[i];
             if (!same) {
-                // mu = floor(b^(2t) / P): sequential division, once per modulus (scratch: q2 = dividend, qp = divisor copy, X = quotient)
+                // mu = floor(b^(2t) / P) < b^(t+1): sequential division, once per modulus (scratch: q2 = dividend,
+                // qp = divisor copy, X = quotient)
                 for (int i = 0; i < 2 * t + 2; ++i) S.q2[i] = 0;
                 S.q2[2 * t] = 1;
                 for (int i = 0; i < t; ++i) S.qp[i] = S.P[i];
                 for (int i = 0; i < 2 * t + 1; ++i) S.X[i] = 0;
                 bd_knuth_div(S.q2, 2 * t, S.qp, t, S.X);
-                if (S.X[t + 1] != 0) {            // P = b^(t-1) exactly: the reciprocal needs t + 2 words - sequential path
-                    S.mode = 0;
-                    S.t_cached = -1;
-                } else {
-                    for (int i = 0; i <= t; ++i) S.mu[i] = S.X[i];
-                    for (int i = 0; i < t; ++i) S.Pc[i] = S.P[i];
-                    S.t_cached = t;
-                }
+                for (int i = 0; i <= t; ++i) S.mu[i] = S.X[i];
+                for (int i = 0; i < t; ++i) S.Pc[i] = S.P[i];
+                S.t_cached = t;
             }
         }
     }
